@@ -16,7 +16,7 @@ at ~4 frames/token (~1022 frames = 11.9 s of audio, a trained model's speech rat
             inputs and D2H of the waveform inside the timed region
   roofline  Generator stage (>99 % of FLOPs): algorithmic layer-boundary bytes (SURVEY.md section 8d: 6 830 852 B per frame) /
             device time of the stage measured with CUDA events inside the timed steps, against MEASURED_PEAKS.json
-  cpu_baseline  the CPU oracle port of the reference (oracle/vits2_oracle.py; /root/reference does not exist on the GPU
+  cpu_baseline  the CPU oracle port of the reference (oracle/vits2_oracle.py; the reference itself does not exist on the GPU
             box) on the host cores, on the SAME utterance
   extras    config2_length_scale_1, config3_batched (B=32, per-stage ms), config5_generator (F=1024 + F/B roofline sweep),
             flow_wn (config 2 with use_transformer_flow=False), and at N>1 config4_sharded (length-bucketed ragged batches
@@ -61,7 +61,7 @@ def peaks():
     if os.path.isfile(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "data sheet (H100 SXM HBM3)"
 
 
 def build_id(only=None):
@@ -84,7 +84,7 @@ def generator_build_id():
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons sampled DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -191,7 +191,7 @@ def cpu_oracle_rate(cfg, sd, budget_s=25.0, max_iters=3):
 def config_dict(frames, world=1, precision=None, parallelism="single GPU"):
     d = {"workload": WORKLOAD_NAME, "global_batch": world * WORKLOAD["B"], "T": WORKLOAD["T"], "length_scale": LENGTH_SCALE_CAL,
          "frames_per_utterance": frames, "audio_seconds_per_utterance": frames * HOP / SR, "parallelism": parallelism,
-         "l2": "no explicit flush: the working set of one step is far beyond the 126 MB L2 (ncu: the Generator alone moves 2.2 GB through DRAM per step, profiles/r02m_generator_traffic.json)"}
+         "l2": "no explicit flush: the working set of one step (Generator activations of ~1000 frames x 512 hop) is far beyond the 50 MB L2"}
     if precision:
         d["precision"] = precision
     return d
@@ -253,6 +253,15 @@ def time_resident(eng, d_inp, d_nw, d_nz, kw, steps, warmup, dev):
     return ms / steps, fr / steps, {k: float(np.mean(v)) for k, v in st.items()}, (eng.launch_count - l0) / steps, Fm[0]
 
 
+def dump_outputs(out_dir, wave, y_lengths):
+    """The arrays the timed path handed its caller in the last step, as .npy files (inputs are seeded: two builds of the project can
+    be compared output for output): wave.npy = the waveform batch [B, 1, samples] (float32, samples past an utterance's length are
+    padding), y_samples.npy = the valid samples of each utterance (y_lengths * hop, float64)."""
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "wave.npy"), wave.detach().float().cpu().numpy())
+    np.save(os.path.join(out_dir, "y_samples.npy"), np.asarray(torch.as_tensor(y_lengths).cpu(), dtype=np.float64).reshape(-1) * HOP)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -261,6 +270,8 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--precision", default=os.environ.get("BV2_PRECISION", "fp16"), choices=["fp32", "tf32", "fp16g", "fp16"])
     ap.add_argument("--cpu-baseline-steps", type=int, default=3)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step returned (waveform batch, per-utterance sample counts) as DIR/<name>.npy")
     ap.add_argument("--extras", type=int, default=1, help="0: headline line only (config2_length_scale_1, config3, config5, flow_wn, config4 skipped)")
     ap.add_argument("--exchange", default="p2p", choices=["p2p", "nccl", "none"],
                     help="N>1: how the finished waveforms reach rank 0 inside the timed region (see step_resident)")
@@ -317,6 +328,8 @@ def main():
                 print(f"[bench] peer slab unavailable ({ex}); using the NCCL gather", file=sys.stderr, flush=True)
             exchange = "nccl"
 
+    last_out = [None, None]  # (waveform batch, per-utterance frame counts) of the latest step_resident()
+
     def step_resident():
         ylen, F = eng.infer_begin(d_inp["x"], d_inp["x_lengths"], d_inp["sid"], d_inp["tone"], d_inp["language"], d_inp["bert"],
                                   d_inp["ja_bert"], d_inp["en_bert"], d_nw, INFER_KW["noise_scale_w"], INFER_KW["length_scale"],
@@ -333,6 +346,7 @@ def main():
             o, attn, y_mask, aux = eng.infer_finish(B, T, F, d_nz, INFER_KW["noise_scale"], want_attn=False)
             if exchange == "nccl":
                 gather_waveforms(o, torch.as_tensor(ylen, device=o.device) * HOP, dst=0)
+        last_out[:] = [o, ylen]
         return int(ylen.sum()), o
 
     def step_e2e():
@@ -400,6 +414,8 @@ def main():
     clocks = sampler.stop() if rank == 0 else None
     launches = eng.launch_count - l0
     flow_ms, enc_ms = float(np.mean(flow_l)), float(np.mean(enc_l))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *last_out)  # the last timed step
     # ---------------- end to end through the public API with host buffers
     for _ in range(args.warmup):
         step_e2e()
@@ -479,9 +495,10 @@ def main():
         g_ms = float(np.mean(gen_ms))
         traffic, traffic_note = None, "no dram__bytes capture for this build (profiles/*_generator_traffic.json build_id mismatch or absent)"
         bid = build_id()
-        for name in sorted(os.listdir(os.path.join(ROOT, "profiles")), reverse=True):
+        pdir = os.path.join(ROOT, "profiles")
+        for name in (sorted(os.listdir(pdir), reverse=True) if os.path.isdir(pdir) else []):
             if name.endswith("_generator_traffic.json"):
-                tj = json.load(open(os.path.join(ROOT, "profiles", name)))
+                tj = json.load(open(os.path.join(pdir, name)))
                 if tj.get("build_id") == bid or tj.get("generator_build_id") == generator_build_id():  # dram__bytes_read+write summed over the Generator launches of one ncu capture (per frame)
                     traffic = tj["generator_dram_bytes_per_frame"] * fpu
                     traffic_note = f"profiles/{name} (" + ("same build" if tj.get("build_id") == bid else "same Generator sources") + ")"

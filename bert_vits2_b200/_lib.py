@@ -1,5 +1,5 @@
 """Build + ctypes binding of libbv2.so (C ABI in include/bv2.h).  No CPU fallback: importing works without
-a GPU (so CPU-only hosts can inspect the ABI), but every compute entry point needs an sm_100 device."""
+a GPU (so CPU-only hosts can inspect the ABI), but every compute entry point needs an sm_90 (H100) device."""
 from __future__ import annotations
 
 import ctypes as C
@@ -14,7 +14,7 @@ TUNING_LIB_PATH = os.path.join(HERE, "libbv2_tuning.so")  # development build (-
 SOURCES = [os.path.join(HERE, "csrc", "engine.cu")]
 HEADERS = sorted(os.path.join(HERE, "csrc", f) for f in os.listdir(os.path.join(HERE, "csrc")) if f.endswith(".cuh")) + [
     os.path.join(ROOT, "include", "bv2.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
 MAX_UPS, MAX_RK, MAX_DIL = 8, 4, 4
 
@@ -79,7 +79,7 @@ def needs_build() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False, tuning: bool = False) -> str:
-    """Compile libbv2.so in-tree for sm_100a with nvcc (cross-compiles without a GPU).
+    """Compile libbv2.so in-tree for sm_90a with nvcc (cross-compiles without a GPU).
     tuning=True builds libbv2_tuning.so instead (same sources, -DBV2_TUNING); it is only ever loaded when BV2_LIB points at it."""
     with _lock:
         out = TUNING_LIB_PATH if tuning else LIB_PATH

@@ -1,4 +1,4 @@
-// Common device/host helpers for libbv2 (sm_100a only).
+// Common device/host helpers for libbv2 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -13,8 +13,8 @@ namespace bv2 {
 // Activation layout used by every internal buffer ("c4"): [B][C/4][T][4] fp32 -- four consecutive
 // channels of one time step form one 16-byte element; time is the next-fastest dimension.  Rationale
 // (DESIGN.md): (1) a time-shifted window of a [C/4][T][4] tile is a pure 16-byte-granular address
-// offset, so the k taps of a dilated Conv1d become k tcgen05 smem-descriptor start addresses over ONE
-// staged tile (K-major, no-swizzle canonical layout with SBO=128 B); (2) TMEM epilogues (one thread per
+// offset, so the k taps of a dilated Conv1d become k wgmma smem-descriptor start addresses over ONE
+// staged tile (K-major, no-swizzle canonical layout with SBO=128 B); (2) accumulator-image epilogues (one thread per
 // time row, channels in registers) store 16-byte vectors that are contiguous across a warp.
 struct Act {
     float* p = nullptr;

@@ -16,8 +16,8 @@
 #include "common.cuh"
 #include "kernels_simt.cuh"
 #include "tc_conv.cuh"
-#include "tc_attn.cuh"
 #include "tc_gen.cuh"
+#include "tc_attn.cuh"
 #include "kernels_tok.cuh"
 
 namespace bv2 {
@@ -50,8 +50,7 @@ public:
     void reset() { off_ = 0; }
     // Sticky high-water mark: the arena only ever grows, and when it must it grows to 1.5x the request (the frame count of an
     // utterance varies with the duration noise), so a steady workload allocates during its first call(s) and never again.
-    // Regrowth is a device-wide sync + cudaFree + cudaMalloc (round 1 measured it inside a timed e2e loop: 10.4 vs 8.4 ms per
-    // step at N=4); bv2_reserve() sizes the arenas up front so that serving loops never hit it.
+    // Regrowth is a device-wide sync + cudaFree + cudaMalloc; bv2_reserve() sizes the arenas up front so that serving loops never hit it.
     void ensure(size_t bytes) {
         if (bytes <= cap_) return;
         bytes += bytes / 2;
@@ -89,7 +88,7 @@ struct bv2_engine {
     bool finalized = false;
     std::vector<void*> dev_allocs;
     int64_t launches = 0;
-    int num_sms = 148;
+    int num_sms = 132;
 
     // ---- device weights
     float *emb = nullptr, *temb = nullptr, *lemb = nullptr, *emb_g = nullptr;
@@ -123,9 +122,8 @@ struct bv2_engine {
         for (int i = 0; i < 4; i++) { BV2_CUDA(cudaStreamCreateWithFlags(&side[i], cudaStreamNonBlocking)); BV2_CUDA(cudaEventCreateWithFlags(&ev_rb[i], cudaEventDisableTiming)); }
         BV2_CUDA(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
     }
-    int flow_tc = 0;       // 0 SIMT fp32, 1 TF32 tcgen05, 2 FP16 tcgen05 + fused attention (finalize)
+    int flow_tc = 0;       // 0 SIMT fp32, 1 TF32 wgmma, 2 FP16 wgmma + fused attention (finalize)
     int use_g2 = 0;        // FP16 Generator on 16-bit activation tensors (tc_gen.cuh)
-    AttnMnConv attn_mn;    // MN-major descriptor convention of the attention's V operand
     bool profiling = false;
     struct StageEv { cudaEvent_t a = nullptr, b = nullptr; bool rec = false; };
     std::map<std::string, StageEv> stage_ev;
@@ -157,7 +155,7 @@ struct bv2_engine {
         if (it == host.end()) throw Error(BV2_ERR_STATE, "missing weight: " + k);
         return it->second;
     }
-    // ---- weight arena.  Every device-resident weight image (SIMT packs, tcgen05 stage images, embeddings, LayerNorm vectors)
+    // ---- weight arena.  Every device-resident weight image (SIMT packs, wgmma stage images, embeddings, LayerNorm vectors)
     // lives in ONE allocation filled by ONE cudaMemcpy.  build_weights() runs twice: a measuring pass (sizes only, packing
     // loops skipped) and the real pass that writes into a host mirror at the same offsets.  bv2_save_packed() dumps that
     // arena; bv2_load_packed() re-runs the structure pass with the packing loops skipped and copies the file in (SURVEY 8f.4).
@@ -416,7 +414,7 @@ struct bv2_engine {
         if (h_err && *reinterpret_cast<volatile int*>(h_err)) {
             *h_err = 0;
             tc_clear_error();
-            throw Error(BV2_ERR_INTERNAL, "device-side barrier timeout in a tcgen05 kernel (results of this call are invalid)");
+            throw Error(BV2_ERR_INTERNAL, "device-side barrier timeout in a wgmma kernel (results of this call are invalid)");
         }
     }
 };
@@ -485,9 +483,8 @@ void bv2_engine::build_weights() {
     const bv2_config& c = cfg;
     const int H = c.hidden_channels, I = c.inter_channels;
     std::vector<float> gw, gb;
-    // Precision policy: stages that feed ceil(durations) never run on the tensor-core path.  Error-compensated 3xTF32
-    // was measured in round 1: the tcgen05 FP32 accumulator truncates, so the error grows linearly with the reduction length
-    // (~6.6e-8 per accumulated product: 1.5e-4 at Cin*K = 2304) and misses the fp32-class accuracy ceil() needs.  These
+    // Precision policy: stages that feed ceil(durations) never run on the tensor-core path: a TF32 / FP16 product carries an 11-bit
+    // significand, so the error grows with the reduction length and misses the fp32-class accuracy ceil() needs.  These
     // stages therefore stay on FP32 FMA (SIMT) in every engine (x3 = 0: no tensor-core weight image is packed for them).
     const int x3 = 0;
     // ---- enc_p (reference models.py:333-375)
@@ -535,7 +532,7 @@ void bv2_engine::build_weights() {
     // ---- flow (reference models.py:82-145 / 403-445): Flip folded into pre/post channel order
     const int half = I / 2, n = c.n_flows;
     flows.resize(n);
-    // generator_precision: 0 = fp32 SIMT everywhere; 1 = TF32 tcgen05 (flow + Generator); 2 = FP16-operand tcgen05 Generator
+    // generator_precision: 0 = fp32 SIMT everywhere; 1 = TF32 wgmma (flow + Generator); 2 = FP16-operand wgmma Generator
     // (same 11-bit significand as TF32, fp32 accumulate, fp32 activations in HBM) + TF32 flow
     // 3 = FP16 operands in the flow too, with the fused attention kernel (tc_attn.cuh)
     const int tc = c.generator_precision == 3 ? 2 : (c.generator_precision ? 1 : 0);
@@ -673,7 +670,7 @@ void bv2_engine::run_encoder(const EncoderW& E, Act x, const int* lens, const fl
             Act att16; att16.B = B; att16.C = H; att16.T = T; att16.p = ws.alloc((size_t)B * H * T / 2);
             tc_out_f16 = 1;
             conv(L.qkv, x, qkv16, s, ConvArgs(), 0, 0, true);
-            tc_flow_attn(qkv16, att16, L.relk, L.relv, lens, nh, (int)cfg.window_size, s, attn_mn); launches++;
+            tc_flow_attn(qkv16, att16, L.relk, L.relv, lens, nh, (int)cfg.window_size, s, num_sms); launches++;
             {   // x = norm_1(x + conv_o(att)): LayerNorm runs in the conv's tail; the residual tile is staged in shared memory by TMA (small grids)
                 // or pre-loaded into the accumulator (more CTAs than SMs)
                 ConvArgs ao; ao.res = x.p; ao.res_mode = 1; ao.res_C_total = H;
@@ -683,8 +680,7 @@ void bv2_engine::run_encoder(const EncoderW& E, Act x, const int* lens, const fl
             ws.release(mk);
             {
                 // FFN hidden tensor as the 16-bit operand image of conv_2 (relu and x_mask applied by conv_1's tail, the conv's zero padding
-                // cleared in the staged tile): conv_2 runs without an operand prologue -- the fp32 -> f16 conversion of its 768-channel
-                // input was the whole MMA phase (1.7 us per 64-channel chunk, profiles/r02g_flow_conv_timelines.log)
+                // cleared in the staged tile): conv_2 runs without an operand prologue (no fp32 -> f16 conversion of its 768-channel input)
                 Act f16 = f;  // same workspace block, half of it used
                 ConvArgs a1; a1.in_mask = 1; a1.act = 1; a1.out_mask = 1; a1.lens = lens;
                 tc_out_f16 = 1;
@@ -729,7 +725,7 @@ void bv2_engine::run_encoder(const EncoderW& E, Act x, const int* lens, const fl
         conv(L.qkv, x, qkv, s, ConvArgs(), 0, 0, tc);
         tc_out_tf32 = 0;
         if (tc) {
-            // tensor-core attention: S = Q.K^T (tcgen05) -> softmax + relative terms (SIMT) -> att += P.V (tcgen05)
+            // tensor-core attention: S = Q.K^T (wgmma) -> softmax + relative terms (SIMT) -> att += P.V (wgmma)
             const size_t mk = ws.used();
             const int Fp = (T + 127) / 128 * 128;
             Act S = ws.act(B * nh, Fp, T);
@@ -965,7 +961,6 @@ void bv2_engine::run_generator(Act z, const int* lens, const float* gdec, int g_
     ConvArgs a; a.bias_b = gdec; a.bias_b_stride = g_stride;
     if (lens) { a.in_mask = 1; a.lens = lens; }
     const bool tc = cfg.generator_precision != 0;
-    const int pair_persist = tune_env("BV2_PAIR_PERSIST", 32);  // max C for the fused ResBlock pair kernel (0 disables)
     conv(conv_pre, z, x, s, a, 0, 0, tc);
     const int nk = cfg.n_resblock_kernels, nd = cfg.n_dilations;
     BV2_CHECK(nk <= 4, "at most 4 resblock kernels");
@@ -997,15 +992,6 @@ void bv2_engine::run_generator(Act z, const int* lens, const float* gdec, int g_
             for (int d = 0; d < nd; d++) {
                 const bool last = d == nd - 1;
                 Act nxt = last ? S : (cur.p == ra.p ? rb : ra);
-                if (tc && u.Cout <= pair_persist) {
-                    // fused ResBlock pair: conv1 -> lrelu -> conv2 + residual in one kernel, intermediate in shared memory
-                    // (declines when fewer than 2 CTAs fit per SM: the two-launch path is faster there)
-                    if (last && j > 0) BV2_CUDA(cudaStreamWaitEvent(sj, ev_rb[j - 1], 0));
-                    const float sc = (last && j == nk - 1) ? 1.f / nk : 1.f;
-                    if (tc_pair_persist(R.c1[d].tc, R.c2[d].tc, R.c1[d].b, R.c2[d].b, cur, nxt, R.dil[d], sc, last && j > 0, sj, num_sms)) {
-                        launches++; cur = nxt; continue;
-                    }
-                }
                 if (tc) {
                     TcEpi e1; e1.in_slope = 0.1f; e1.dil = R.dil[d];
                     tc_conv1d(R.c1[d].tc, R.c1[d].b, cur, xt, e1, sj, num_sms); launches++;
@@ -1123,7 +1109,7 @@ static size_t persist_bytes_for(const bv2_config& c, int B, int T, int gproj_n) 
 
 extern "C" {
 
-const char* bv2_version(void) { return "bv2-b200 0.1 (sm_100a)"; }
+const char* bv2_version(void) { return "bv2-b200 0.1 (sm_90a)"; }
 
 int bv2_create(bv2_engine** out, const bv2_config* cfg, int cuda_device) {
     if (!out || !cfg) return BV2_ERR_ARG;
@@ -1132,7 +1118,7 @@ int bv2_create(bv2_engine** out, const bv2_config* cfg, int cuda_device) {
     if (cudaGetDeviceCount(&n) != cudaSuccess || cuda_device < 0 || cuda_device >= n) return BV2_ERR_CUDA;
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, cuda_device) != cudaSuccess) return BV2_ERR_CUDA;
-    if (prop.major != 10) return BV2_ERR_CUDA;  // sm_100a only: no fallback path exists
+    if (prop.major != 9) return BV2_ERR_CUDA;  // sm_90a only: no fallback path exists
     bv2_engine* e = new bv2_engine();
     e->cfg = *cfg;
     e->device = cuda_device;
@@ -1165,7 +1151,7 @@ int bv2_finalize(bv2_engine* e) {
 }
 
 // ---- packed engine weight file (SURVEY.md section 8f.4; the reference's counterpart is compress_model.py:44-53, which only drops enc_q and
-// casts to fp16): header | reference state_dict key/shape table | arena image (weight-norm folded, Flip folded, SIMT + tcgen05 packs).
+// casts to fp16): header | reference state_dict key/shape table | arena image (weight-norm folded, Flip folded, SIMT + wgmma packs).
 namespace {
 struct PackHeader {
     char magic[8];

@@ -1,6 +1,6 @@
 // fp32 SIMT kernels of the VITS2 infer path, all on the c4 activation layout (common.cuh).
 // These are (1) the exact-fp32 path for everything that feeds ceil(durations) (text encoder, SDP, DP:
-// SURVEY.md §7 H1) and (2) the fallback/baseline for the stages whose dense contractions run on tcgen05
+// SURVEY.md §7 H1) and (2) the fallback/baseline for the stages whose dense contractions run on wgmma
 // (tc_conv.cuh).  Each kernel cites the reference op sequence it replaces.
 #pragma once
 #include "common.cuh"
@@ -929,7 +929,7 @@ __global__ void __launch_bounds__(256) k_conv_post_tanh(const float* __restrict_
 }
 
 // ------------------------------------------------------------------------------------------------
-// Tensor-core attention, middle stage (the Q.K^T and P.V contractions run on tcgen05: tc_attn_qk / tc_attn_pv).
+// Tensor-core attention, middle stage (the Q.K^T and P.V contractions run on wgmma: tc_attn_qk / tc_attn_pv).
 // S: c4 over keys [Z = B*heads][Fp/4][T queries][4] holding q_i.k_j; rewritten in place with the softmax
 // probabilities of reference attentions.py:280-308 (banded relative-key logits added here, keys >= len excluded,
 // rows of invalid queries and columns >= len zeroed so the P.V GEMM can run over the padded key range).
@@ -1067,7 +1067,7 @@ __global__ void __launch_bounds__(32 * NP) k_attn_softmax(const float* __restric
     }
 }
 
-// V^T pack for the P.V GEMM: vt[z][Fp/32][8][DK][4] (the UMMA K-major B-operand image, K = keys), zeros for keys >= len.
+// V^T pack for the P.V GEMM: vt[z][Fp/32][8][DK][4] (the wgmma K-major B-operand image, K = keys), zeros for keys >= len.
 template <int DK>
 __global__ void k_pack_vt(const float* __restrict__ qkv, float* __restrict__ vt, int H, int heads, int T, int Fp, const int* __restrict__ lens) {
     pdl_wait();

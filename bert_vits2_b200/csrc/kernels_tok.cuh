@@ -1,5 +1,5 @@
 // Fused FP32 kernels of the token-rate stage (text encoder, SDP, DP: everything that feeds ceil(durations) stays on FP32 FMA,
-// SURVEY.md section 7 H1).  At T ~ 256 tokens this stage is pure launch / dependency latency (round 1: ~110 launches of 5-40 us),
+// SURVEY.md section 7 H1).  At T ~ 256 tokens this stage is pure launch / dependency latency (~110 small launches unfused),
 // so the kernels here trade launches for on-chip fusion: a whole layer per launch, weights staged in shared memory by TMA.
 #pragma once
 #include "kernels_simt.cuh"

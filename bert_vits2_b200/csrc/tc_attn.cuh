@@ -1,27 +1,28 @@
-// Fused windowed relative-position multi-head self-attention of the flow's transformer layers on tcgen05
+// Fused windowed relative-position multi-head self-attention of the flow's transformer layers on Hopper wgmma
 // (reference attentions.py:263-322 via attentions.py:103-120, called 16x per infer by TransformerCouplingBlock, models.py:82-145):
 //     scores[i,j] = q_i.k_j + [|j-i| <= w] q_i.Ek[j-i+w]      (q pre-scaled by 1/sqrt(dk) in the QKV projection weights)
 //     p = softmax_j(scores, keys j >= len excluded)            out_i = sum_j p_ij v_j + sum_r p_{i,i+r-w} Ev[r]
-// One CTA = 128 queries of one (batch, head).  S = Q.K^T lives in TMEM (double-buffered), the softmax warps turn it into the
-// FP16 A-operand image P in shared memory, P.V accumulates into a second TMEM accumulator: neither S nor P ever reaches
-// HBM/L2 (round 1: S/P round trips of 4*F^2*4 B per head-layer through three kernels + a V^T pack = 95 us per layer).
+// One CTA = 128 queries of one (batch, head), split over two consumer warpgroups of 64 query rows each.  S = Q.K^T of a key tile
+// is a register accumulator of the warpgroup (wgmma, both operands in shared memory); the softmax runs on that fragment and the
+// probabilities go to the P.V wgmma straight from registers (the accumulator fragment of S for 16 key columns is the A-operand
+// fragment of one k-step), so neither S nor P is ever stored; O = P.V accumulates in registers across the key tiles.
 //
 // Operands are the 16-bit c8 tensors the QKV projection's epilogue writes ([B][3H/8][T][8 halves]):
 //   * a [dk/8][rows][8] tile of q or k IS the K-major no-swizzle operand image (TMA copies it straight from global memory);
 //   * v needs no transposition either: [dk/8][keys][8] is the MN-major no-swizzle image of the [keys x dk] B operand
-//     (8 keys x 16 bytes = one 128-byte core matrix), selected with the b_major bit of the instruction descriptor.
+//     (8 keys x 16 bytes = one 128-byte core matrix; LBO = stride between 8-key blocks, SBO = stride between 8-channel blocks).
 // Two passes over the key tiles instead of an online softmax: pass A computes the row maxima (Q.K^T + max only), pass B
-// recomputes Q.K^T, exponentiates against the final maximum and feeds P.V -- no accumulator rescaling, i.e. no TMEM
-// read-modify-write in the MMA dependency chain, at the price of 12 extra (cheap, overlapped) MMAs per key tile.
+// recomputes Q.K^T, exponentiates against the final maximum and feeds P.V -- no accumulator rescaling.
 //
-// Key split (B = 1 leaves only 2 heads x F/128 query tiles = 16 CTAs for 148 SMs, each walking every key tile twice): a cluster of
+// Key split (B = 1 leaves only 2 heads x F/128 query tiles = 16 CTAs for 132 SMs, each walking every key tile twice): a cluster of
 // ks CTAs shares a query tile, CTA r handles key tiles r, r + ks, ... with its OWN running maximum, and the partial results
 // (m_r, l_r, relative-value weights, unnormalised P.V rows) are merged flash-decoding style over distributed shared memory:
 //     m = max_r m_r,  w_r = 2^((m_r - m) log2 e),  out = (sum_r w_r O_r + sum_r w_r prel_r . Ev) / sum_r w_r l_r
 // Each CTA parks its partial rows in its own shared memory (the K/V stages are free by then), one cluster barrier, CTA c pulls
 // rows [c*128/ks, (c+1)*128/ks) of every peer (ld.shared::cluster) in fixed rank order -- deterministic -- and writes them.
-// 192 threads: warp 0 TMA producer (Q once, K tiles twice, V tiles once), warp 1 TMEM allocator + MMA issuer,
-// warps 2-5 softmax / epilogue (one thread per query row).
+// Without a key split (ks = 1) the same merge runs on the CTA's own rows.
+// 288 threads: warps 0-7 = two consumer warpgroups (scores, softmax, P.V, parking, merge), warp 8 = TMA producer (Q once, K tiles
+// twice, V tiles once).
 #pragma once
 #include "tc_conv.cuh"
 
@@ -34,7 +35,7 @@ struct AttnParams {
     const int* lens;    // valid length per batch (keys >= len excluded, query rows >= len produce zeros)
     int B, T, H, heads, window;
     int ks;             // key split: a cluster of ks CTAs shares one 128-query tile, CTA r takes key tiles r, r + ks, ... (1 = no cluster)
-    uint32_t idesc_qk, idesc_pv, v_lbo, v_sbo;
+    uint32_t v_lbo, v_sbo;  // MN-major descriptor strides of the V operand
     long long* prof;    // probes only: per-CTA globaltimer stamps [ctas][10]; nullptr in the engine
 };
 
@@ -48,8 +49,8 @@ __device__ __forceinline__ void unpack_h8(const uint4& u, float* f) {
 }  // namespace tc
 
 // Merge of the key splits (flash-decoding style) for one thread: row m of the query tile, 96/KSC channels.  Every distributed-shared-memory
-// load is issued before the first dependent instruction (a ld.shared::cluster round trip is ~0.2 us; interleaved with the arithmetic the 36
-// loads of a 4-way merge ran one after the other: 8.4 us of the 30 us kernel at config 2, profiles/r02j_attn_timeline.log).
+// load is issued before the first dependent instruction (interleaved with the arithmetic, the 36 loads of a 4-way merge would each
+// pay a full distributed-shared-memory round trip one after the other).
 // Peers are combined in fixed rank order: deterministic.
 template <int KSC, int DK>
 __device__ __forceinline__ void attn_merge_rows(uint32_t sK_addr, const float* sEv, int rk, int t, int q0, int len, int T, int nrel, uint4* obase) {
@@ -120,26 +121,24 @@ __device__ __forceinline__ void attn_merge_rows(uint32_t sK_addr, const float* s
 }
 
 template <int DK, int KT>
-__global__ void __launch_bounds__(192, 1) k_flow_attn(AttnParams p) {
+__global__ void __launch_bounds__(288, 1) k_flow_attn(AttnParams p) {
     using namespace tc;
     extern __shared__ __align__(1024) uint8_t smem[];
     constexpr int NG = DK / 8, NREL = 9;
-    constexpr uint32_t QB = DK * 128 * 2, KB = DK * KT * 2, PB = KT * 128 * 2;
+    constexpr uint32_t QB = DK * 128 * 2, KB = DK * KT * 2;
     constexpr float LOG2E = 1.4426950408889634f;
-    static_assert(KT == 128 && DK % 16 == 0 && DK <= 128, "tile shape");
+    static_assert(KT == 128 && DK == 96, "tile shape (wgmma_ss_n128 / wgmma_rs_n96_tb)");
     uint8_t* sQ = smem;
     uint8_t* sK = sQ + QB;
     uint8_t* sV = sK + 2 * KB;
-    uint8_t* sP = sV + 2 * KB;
-    float* sEk = reinterpret_cast<float*>(sP + 2 * PB);
+    float* sEk = reinterpret_cast<float*>(sV + 2 * KB);
     float* sEv = sEk + NREL * DK;
-    float* sQrel = sEv + NREL * DK;    // [NREL][128 rows]: q_i . Ek[r] of this CTA's query rows (each thread reads back only its own row)
+    float* sQrel = sEv + NREL * DK;    // [NREL][128 rows]: q_i . Ek[r] of this CTA's query rows
     float* sPrel = sQrel + NREL * 128; // [NREL][128 rows]: p[i, i + r - w], written by the pass-B thread that meets that key
     uint64_t* bars = reinterpret_cast<uint64_t*>(sPrel + NREL * 128);
     const uint32_t bar0 = smem_u32(bars);
     auto BAR = [&](int i) { return bar0 + 8u * (uint32_t)i; };
-    enum { B_QFULL = 0, B_KFULL = 1, B_KEMPTY = 3, B_VFULL = 5, B_VEMPTY = 7, B_SFULL = 9, B_SEMPTY = 11, B_PFULL = 13, B_PEMPTY = 15, B_OFULL = 17, NBARS = 18 };
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + NBARS);
+    enum { B_QFULL = 0, B_KFULL = 1, B_KEMPTY = 3, B_VFULL = 5, B_VEMPTY = 7, NBARS = 9 };
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int KS = p.ks, rk = (int)blockIdx.x % KS;  // cluster dims (KS,1,1): rank in cluster == blockIdx.x % KS
     const int q0 = ((int)blockIdx.x / KS) * 128, h = blockIdx.y, b = blockIdx.z;
@@ -147,33 +146,23 @@ __global__ void __launch_bounds__(192, 1) k_flow_attn(AttnParams p) {
     const int w = p.window, nrel = 2 * w + 1;
     auto gtimer = [] { long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; };
     long long* prof = p.prof ? p.prof + ((size_t)(blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 10 : nullptr;
-    const bool stamp = prof && threadIdx.x == 64;  // first softmax thread
-    if (prof && threadIdx.x == 0) prof[0] = gtimer();
+    const bool stamp = prof && threadIdx.x == 0;
+    if (stamp) prof[0] = gtimer();
 
     if (threadIdx.x == 0) {
-        mbar_init(BAR(B_QFULL), 1); mbar_init(BAR(B_OFULL), 1);
-        for (int i = 0; i < 2; i++) {
-            mbar_init(BAR(B_KFULL + i), 1); mbar_init(BAR(B_KEMPTY + i), 1); mbar_init(BAR(B_VFULL + i), 1); mbar_init(BAR(B_VEMPTY + i), 1);
-            mbar_init(BAR(B_SFULL + i), 1); mbar_init(BAR(B_SEMPTY + i), 128); mbar_init(BAR(B_PFULL + i), 128); mbar_init(BAR(B_PEMPTY + i), 1);
-        }
+        mbar_init(BAR(B_QFULL), 1);
+        for (int i = 0; i < 2; i++) { mbar_init(BAR(B_KFULL + i), 1); mbar_init(BAR(B_KEMPTY + i), 2); mbar_init(BAR(B_VFULL + i), 1); mbar_init(BAR(B_VEMPTY + i), 2); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
     }
     // V tiles are loaded with partial row counts at the end of the sequence: rows never written must hold finite values (they meet
     // p = 0 in the P.V MMA), so both V stages start zeroed; later partial loads leave finite rows of an earlier tile behind.
     for (int i = threadIdx.x; i < (int)(2 * KB / 16); i += blockDim.x) reinterpret_cast<uint4*>(sV)[i] = make_uint4(0u, 0u, 0u, 0u);
     for (int i = threadIdx.x; i < nrel * DK; i += blockDim.x) { sEk[i] = p.rel_k[i]; sEv[i] = p.rel_v[i]; }
     fence_async_smem();
-    fence_before();
     __syncthreads();
-    fence_after();
-    const uint32_t tmem = __shfl_sync(0xffffffffu, *tmem_slot, 0);  // shfl: a warp-uniform value for ptxas (uniform registers in the MMA issuer)
     asm volatile("griddepcontrol.wait;" ::: "memory");
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    if (prof && threadIdx.x == 0) prof[1] = gtimer();
+    if (stamp) prof[1] = gtimer();
 
     const int len = min(p.lens ? p.lens[b] : p.T, p.T);
     const int NT_all = q0 < len ? (len + KT - 1) / KT : 0;  // key tiles that hold at least one valid key (same for the whole cluster)
@@ -181,8 +170,9 @@ __global__ void __launch_bounds__(192, 1) k_flow_attn(AttnParams p) {
     const uint4* qbase = p.qkv + ((size_t)b * 3 * H8 + (size_t)h * NG) * p.T;
     const uint4* kbase = qbase + (size_t)H8 * p.T;
     const uint4* vbase = kbase + (size_t)H8 * p.T;
+    uint4* obase = p.att + ((size_t)b * H8 + (size_t)h * NG) * p.T;
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (NT > 0) {
             const int nq = min(128, p.T - q0);
             if (lane == 0) mbar_expect_tx(BAR(B_QFULL), (uint32_t)nq * 16u * NG);
@@ -209,238 +199,168 @@ __global__ void __launch_bounds__(192, 1) k_flow_attn(AttnParams p) {
                 }
             }
         }
-    } else if (warp == 1) {
-        if (NT > 0) {  // all 32 lanes run the issue loop convergently; elect_one() guards the MMAs / commits
-            mbar_wait_u(BAR(B_QFULL), 0);
-            auto qk = [&](int s) {  // S[s&1] = Q . K_tile^T
-                const int st = s & 1;
-                mbar_wait_u(BAR(B_KFULL + st), (s >> 1) & 1);
-                mbar_wait_u(BAR(B_SEMPTY + st), ((s >> 1) & 1) ^ 1);
-                fence_after();
-                uint64_t ad = make_desc(smem_u32(sQ), 128u * 16u, 128u);
-                uint64_t bd = make_desc(smem_u32(sK) + (uint32_t)st * KB, (uint32_t)KT * 16u, 128u);
-                const uint32_t d = tmem + (uint32_t)(st * KT);
-#pragma unroll
-                for (int kk = 0; kk < DK / 16; kk++, ad += 2u * 128u, bd += 2u * KT) umma_e<1>(d, ad, bd, p.idesc_qk, kk ? 1u : 0u);
-                umma_commit_e(BAR(B_KEMPTY + st));
-                umma_commit_e(BAR(B_SFULL + st));
-            };
-            qk(0);
-            for (int s = 0; s < 2 * NT; s++) {
-                if (s + 1 < 2 * NT) qk(s + 1);  // the next tile's scores are computed while the softmax warps work on this one
-                if (s >= NT) {
-                    const int j = s - NT, pb = j & 1;
-                    mbar_wait_u(BAR(B_PFULL + pb), (j >> 1) & 1);
-                    mbar_wait_u(BAR(B_VFULL + pb), (j >> 1) & 1);
-                    fence_after();
-                    uint64_t ad = make_desc(smem_u32(sP) + (uint32_t)pb * PB, 128u * 16u, 128u);
-                    uint64_t bd = make_desc(smem_u32(sV) + (uint32_t)pb * KB, p.v_lbo, p.v_sbo);
-                    const uint32_t d = tmem + 2u * KT;
-#pragma unroll
-                    for (int kk = 0; kk < KT / 16; kk++, ad += 2u * 128u, bd += 16u) umma_e<1>(d, ad, bd, p.idesc_pv, (j | kk) ? 1u : 0u);
-                    umma_commit_e(BAR(B_PEMPTY + pb));
-                    umma_commit_e(BAR(B_VEMPTY + pb));
-                    if (j == NT - 1) umma_commit_e(BAR(B_OFULL));
-                }
-            }
-        }
+    } else if (NT_all == 0) {  // every query of this tile is padding: zeros (written once per cluster)
+        const int i = q0 + (int)threadIdx.x;
+        if (threadIdx.x < 128 && i < p.T && rk == 0)
+            for (int g = 0; g < NG; g++) obase[(size_t)g * p.T + i] = make_uint4(0u, 0u, 0u, 0u);
     } else {
-        const int q = warp & 3, m = q * 32 + lane, i = q0 + m;
-        const uint32_t trow = tmem + ((uint32_t)(q * 32) << 16);
-        uint4* obase = p.att + ((size_t)b * H8 + (size_t)h * NG) * p.T;
-        if (NT_all == 0) {  // every query of this tile is padding: zeros (written once per cluster)
-            if (i < p.T && rk == 0)
-                for (int g = 0; g < NG; g++) obase[(size_t)g * p.T + i] = make_uint4(0u, 0u, 0u, 0u);
-        } else {
-            float M = -INFINITY, L = 0.f;
-            float prel[NREL];
+        // consumer warpgroup wg owns query rows [64 wg, 64 wg + 64); this thread holds rows r0 and r0 + 8 of the wgmma fragments
+        // and, in each 8-column block, columns cq and cq + 1
+        const int ct = threadIdx.x, wg = ct >> 7, t = ct & 127;
+        const int r0 = 64 * wg + 16 * (t >> 5) + ((t & 31) >> 2), cq = 2 * (t & 3);
+        float M[2] = {-INFINITY, -INFINITY}, L[2] = {0.f, 0.f};
+        float o[DK / 2];
 #pragma unroll
-            for (int r = 0; r < NREL; r++) prel[r] = 0.f;
-            if (NT > 0) {
-            // ---- relative-key logits of this row: qrel[r] = q_i . Ek[r]
-            float qrel[NREL];
-#pragma unroll
-            for (int r = 0; r < NREL; r++) qrel[r] = 0.f;
+        for (int e = 0; e < DK / 2; e++) o[e] = 0.f;
+        if (NT > 0) {
             mbar_wait(BAR(B_QFULL), 0);
-            for (int g = 0; g < NG; g++) {
-                float qf[8];
-                unpack_h8(reinterpret_cast<const uint4*>(sQ)[g * 128 + m], qf);
+            if (ct < 128) {
+                // ---- relative-key logits of row m: qrel[r] = q_i . Ek[r]
+                const int m = ct;
+                float qrel[NREL];
 #pragma unroll
-                for (int r = 0; r < NREL; r++) {
-                    if (r < nrel) {
-                        const float4 e0 = *reinterpret_cast<const float4*>(&sEk[r * DK + g * 8]), e1 = *reinterpret_cast<const float4*>(&sEk[r * DK + g * 8 + 4]);
-                        float a = qrel[r];  // same accumulation order as a scalar loop over the 8 channels
-                        a = fmaf(qf[0], e0.x, a); a = fmaf(qf[1], e0.y, a); a = fmaf(qf[2], e0.z, a); a = fmaf(qf[3], e0.w, a);
-                        a = fmaf(qf[4], e1.x, a); a = fmaf(qf[5], e1.y, a); a = fmaf(qf[6], e1.z, a); a = fmaf(qf[7], e1.w, a);
-                        qrel[r] = a;
+                for (int r = 0; r < NREL; r++) qrel[r] = 0.f;
+                for (int g = 0; g < NG; g++) {
+                    float qf[8];
+                    unpack_h8(reinterpret_cast<const uint4*>(sQ)[g * 128 + m], qf);
+#pragma unroll
+                    for (int r = 0; r < NREL; r++) {
+                        if (r < nrel) {
+                            const float4 e0 = *reinterpret_cast<const float4*>(&sEk[r * DK + g * 8]), e1 = *reinterpret_cast<const float4*>(&sEk[r * DK + g * 8 + 4]);
+                            float a = qrel[r];  // same accumulation order as a scalar loop over the 8 channels
+                            a = fmaf(qf[0], e0.x, a); a = fmaf(qf[1], e0.y, a); a = fmaf(qf[2], e0.z, a); a = fmaf(qf[3], e0.w, a);
+                            a = fmaf(qf[4], e1.x, a); a = fmaf(qf[5], e1.y, a); a = fmaf(qf[6], e1.z, a); a = fmaf(qf[7], e1.w, a);
+                            qrel[r] = a;
+                        }
                     }
+                }
+#pragma unroll
+                for (int r = 0; r < NREL; r++) { sQrel[r * 128 + m] = qrel[r]; sPrel[r * 128 + m] = 0.f; }
+            }
+            asm volatile("bar.sync 1, 256;" ::: "memory");  // both consumer warpgroups: the qrel / prel tables are complete
+            if (stamp) prof[2] = gtimer();
+            const uint64_t qd = make_desc(smem_u32(sQ), 128u * 16u, 128u) + (uint64_t)(64 * wg);  // 64 rows further = 8 core-matrix groups
+            // S (64 rows x KT keys of this warpgroup) = Q . K_tile^T, then the K stage goes back to the producer
+            auto scores = [&](int s, float* c) {
+                const int st = s & 1;
+                mbar_wait(BAR(B_KFULL + st), (s >> 1) & 1);
+#pragma unroll
+                for (int e = 0; e < KT / 2; e++) c[e] = 0.f;
+                const uint64_t kd = make_desc(smem_u32(sK) + (uint32_t)st * KB, (uint32_t)KT * 16u, 128u);
+                wgmma_fence();
+#pragma unroll
+                for (int kk = 0; kk < DK / 16; kk++) wgmma_ss_n128(c, qd + (uint64_t)(kk * 2 * 128), kd + (uint64_t)(kk * 2 * KT));
+                wgmma_commit();
+                wgmma_wait0();
+                asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+                if (t == 0) mbar_arrive(BAR(B_KEMPTY + st));
+            };
+            // ---- pass A: row maxima over the valid keys (of this CTA's key tiles)
+            for (int s = 0; s < NT; s++) {
+                const int k0 = (rk + KS * s) * KT, nvalid = len - k0;
+                const bool band = (k0 <= q0 + 127 + w) && (k0 + KT - 1 >= q0 - w);
+                float c[KT / 2];
+                scores(s, c);
+#pragma unroll
+                for (int e = 0; e < KT / 2; e++) {
+                    const int hr = (e >> 1) & 1, row = r0 + 8 * hr, col = 8 * (e >> 2) + cq + (e & 1);
+                    float x = c[e];
+                    if (band) { const int d = k0 + col - (q0 + row) + w; if ((unsigned)d < (unsigned)nrel) x += sQrel[d * 128 + row]; }
+                    if (col < nvalid) M[hr] = fmaxf(M[hr], x);
                 }
             }
-            // per-row tables in shared memory, indexed by the relative position d = j - i + w (a per-lane value): one predicated LDS / STS per
-            // in-band element instead of a 9-way select chain over registers (the chains were ~8x the plain softmax path per element and
-            // ran on every element of the in-band chunks: 3.6 us of pass A and 5.7 us of pass B on the CTA that owns the diagonal tile,
-            // which is the one the whole cluster waits for: profiles/r02m_attn_timeline.log).  [r][row] layout: conflict-free (stride 127 mod 32).
 #pragma unroll
-            for (int r = 0; r < NREL; r++) { sQrel[r * 128 + m] = qrel[r]; sPrel[r * 128 + m] = 0.f; }
-            if (stamp) prof[2] = gtimer();
-            // ---- pass A: row maximum over the valid keys (of this CTA's key tiles)
-            for (int s = 0; s < NT; s++) {
-                const int st = s & 1, k0 = (rk + KS * s) * KT, nvalid = len - k0;
-                const bool band = (k0 <= q0 + 127 + w) && (k0 + KT - 1 >= q0 - w);
-                mbar_wait(BAR(B_SFULL + st), (s >> 1) & 1);
-                fence_after();
-                for (int c0 = 0; c0 < KT; c0 += 32) {
-                    uint32_t v[32];
-                    tmem_ld32(trow + (uint32_t)(st * KT + c0), v);
-                    tmem_wait_ld();
-                    // relative-key terms only in the 32-column chunks that can hold a key within +-w of one of THIS warp's 32 query rows
-                    // (warp-uniform; the band logic costs ~8x the plain path per element and used to run on every chunk of an in-band tile)
-                    if (band && (k0 + c0 + 31 >= q0 + 32 * q - w) && (k0 + c0 <= q0 + 32 * q + 31 + w)) {
-#pragma unroll
-                        for (int e = 0; e < 32; e++) {
-                            const int d = k0 + c0 + e - i + w;
-                            float x = __uint_as_float(v[e]);
-                            if ((unsigned)d < (unsigned)nrel) x += sQrel[d * 128 + m];
-                            if (c0 + e < nvalid) M = fmaxf(M, x);
-                        }
-                    } else {
-#pragma unroll
-                        for (int e = 0; e < 32; e++)
-                            if (c0 + e < nvalid) M = fmaxf(M, __uint_as_float(v[e]));
-                    }
-                }
-                fence_before();
-                mbar_arrive(BAR(B_SEMPTY + st));
+            for (int hr = 0; hr < 2; hr++) {
+                M[hr] = fmaxf(M[hr], __shfl_xor_sync(0xffffffffu, M[hr], 1));
+                M[hr] = fmaxf(M[hr], __shfl_xor_sync(0xffffffffu, M[hr], 2));
             }
             if (stamp) prof[3] = gtimer();
-            // ---- pass B: p = exp(s - M) -> FP16 operand image in shared memory; row sum; relative-value weights
-            const float M2 = M * LOG2E;
+            // ---- pass B: p = exp(s - M) in registers -> P.V; row sums; relative-value weights
+            const float M2[2] = {M[0] * LOG2E, M[1] * LOG2E};
             for (int j = 0; j < NT; j++) {
-                const int s = NT + j, st = s & 1, pb = j & 1, k0 = (rk + KS * j) * KT, nvalid = len - k0;
+                const int vs = j & 1, k0 = (rk + KS * j) * KT, nvalid = len - k0;
                 const bool band = (k0 <= q0 + 127 + w) && (k0 + KT - 1 >= q0 - w);
-                mbar_wait(BAR(B_SFULL + st), (s >> 1) & 1);
-                mbar_wait(BAR(B_PEMPTY + pb), ((j >> 1) & 1) ^ 1);
-                fence_after();
-                uint4* P = reinterpret_cast<uint4*>(sP + (size_t)pb * PB);
-                for (int c0 = 0; c0 < KT; c0 += 32) {
-                    uint32_t v[32];
-                    tmem_ld32(trow + (uint32_t)(st * KT + c0), v);
-                    tmem_wait_ld();
-                    float pe[32];
-                    if (band && (k0 + c0 + 31 >= q0 + 32 * q - w) && (k0 + c0 <= q0 + 32 * q + 31 + w)) {
+                float c[KT / 2];
+                scores(NT + j, c);
 #pragma unroll
-                        for (int e = 0; e < 32; e++) {
-                            const int d = k0 + c0 + e - i + w;
-                            float x = __uint_as_float(v[e]);
-                            const bool inb = (unsigned)d < (unsigned)nrel;
-                            if (inb) x += sQrel[d * 128 + m];
-                            pe[e] = (c0 + e < nvalid) ? ex2_approx(fmaf(x, LOG2E, -M2)) : 0.f;
-                            if (inb) sPrel[d * 128 + m] = pe[e];  // key j = i + d - w is met exactly once
-                        }
-                    } else {
-#pragma unroll
-                        for (int e = 0; e < 32; e++) pe[e] = (c0 + e < nvalid) ? ex2_approx(fmaf(__uint_as_float(v[e]), LOG2E, -M2)) : 0.f;
-                    }
-#pragma unroll
-                    for (int g = 0; g < 4; g++) {
-                        uint4 o;
-                        o.x = pack_h2(pe[8 * g], pe[8 * g + 1]); o.y = pack_h2(pe[8 * g + 2], pe[8 * g + 3]);
-                        o.z = pack_h2(pe[8 * g + 4], pe[8 * g + 5]); o.w = pack_h2(pe[8 * g + 6], pe[8 * g + 7]);
-                        P[(size_t)(c0 / 8 + g) * 128 + m] = o;
-                    }
-#pragma unroll
-                    for (int e = 0; e < 32; e++) L += pe[e];
+                for (int e = 0; e < KT / 2; e++) {
+                    const int hr = (e >> 1) & 1, row = r0 + 8 * hr, col = 8 * (e >> 2) + cq + (e & 1);
+                    float x = c[e];
+                    int d = -1;
+                    if (band) { d = k0 + col - (q0 + row) + w; if ((unsigned)d < (unsigned)nrel) x += sQrel[d * 128 + row]; else d = -1; }
+                    const float pe = col < nvalid ? ex2_approx(fmaf(x, LOG2E, -M2[hr])) : 0.f;
+                    if (d >= 0) sPrel[d * 128 + row] = pe;  // key j = i + d - w is met exactly once
+                    L[hr] += pe;
+                    c[e] = pe;
                 }
-                fence_before();
-                fence_async_smem();
-                mbar_arrive(BAR(B_PFULL + pb));
-                mbar_arrive(BAR(B_SEMPTY + st));
+                // the S fragment of key columns [16 kk, 16 kk + 16) is the A fragment of k-step kk
+                uint32_t a[KT / 16][4];
+#pragma unroll
+                for (int kk = 0; kk < KT / 16; kk++) {
+                    a[kk][0] = pack_h2(c[8 * kk], c[8 * kk + 1]); a[kk][1] = pack_h2(c[8 * kk + 2], c[8 * kk + 3]);
+                    a[kk][2] = pack_h2(c[8 * kk + 4], c[8 * kk + 5]); a[kk][3] = pack_h2(c[8 * kk + 6], c[8 * kk + 7]);
+                }
+                mbar_wait(BAR(B_VFULL + vs), (j >> 1) & 1);
+                const uint64_t vd = make_desc(smem_u32(sV) + (uint32_t)vs * KB, p.v_lbo, p.v_sbo);
+                wgmma_fence();
+#pragma unroll
+                for (int kk = 0; kk < KT / 16; kk++) wgmma_rs_n96_tb(o, a[kk], vd + (uint64_t)(16 * kk));  // 16 keys = two 128-byte key blocks
+                wgmma_commit();
+                wgmma_wait0();
+                asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+                if (t == 0) mbar_arrive(BAR(B_VEMPTY + vs));
             }
 #pragma unroll
-            for (int r = 0; r < NREL; r++) prel[r] = sPrel[r * 128 + m];
+            for (int hr = 0; hr < 2; hr++) {
+                L[hr] += __shfl_xor_sync(0xffffffffu, L[hr], 1);
+                L[hr] += __shfl_xor_sync(0xffffffffu, L[hr], 2);
+            }
             if (stamp) prof[4] = gtimer();
-            mbar_wait(BAR(B_OFULL), 0);  // every MMA of this CTA has completed: O is final, the K/V/P stages are free
-            fence_after();
-            if (stamp) prof[5] = gtimer();
-            }  // NT > 0
-            if (KS > 1) {
-                // ---- park this CTA's partial row in its own shared memory (the K stages): [27 float4][128 rows]
-                //      slots 0..23 unnormalised P.V (96 channels), 24 = (m, l, prel0, prel1), 25 = prel2..5, 26 = prel6..8
-                float4* part = reinterpret_cast<float4*>(sK);
-                for (int c0 = 0; c0 < DK; c0 += 32) {
-                    uint32_t v[32];
-                    if (NT > 0) { tmem_ld32(trow + (uint32_t)(2 * KT + c0), v); tmem_wait_ld(); }
-                    else {
-#pragma unroll
-                        for (int e = 0; e < 32; e++) v[e] = 0u;
-                    }
-#pragma unroll
-                    for (int g = 0; g < 8; g++)
-                        part[(size_t)(c0 / 4 + g) * 128 + m] = make_float4(__uint_as_float(v[4 * g]), __uint_as_float(v[4 * g + 1]), __uint_as_float(v[4 * g + 2]), __uint_as_float(v[4 * g + 3]));
-                }
-                part[(size_t)24 * 128 + m] = make_float4(M, L, prel[0], prel[1]);
-                part[(size_t)25 * 128 + m] = make_float4(prel[2], prel[3], prel[4], prel[5]);
-                part[(size_t)26 * 128 + m] = make_float4(prel[6], prel[7], prel[8], 0.f);
-            } else {
-            // ---- epilogue: out = (P.V + sum_r p_rel[r] Ev[r]) / L  -> 16-bit c8 (the operand image of conv_o)
-            const float inv = (i < len && L > 0.f) ? 1.f / L : 0.f;
-            for (int c0 = 0; c0 < DK; c0 += 32) {
-                uint32_t v[32];
-                tmem_ld32(trow + (uint32_t)(2 * KT + c0), v);
-                tmem_wait_ld();
-                float o[32];
-#pragma unroll
-                for (int e = 0; e < 32; e++) o[e] = __uint_as_float(v[e]);
-#pragma unroll
-                for (int r = 0; r < NREL; r++) {
-                    if (r < nrel) {
-                        const float pw = prel[r];
-                        const float* ev = &sEv[r * DK + c0];
-#pragma unroll
-                        for (int e = 0; e < 32; e++) o[e] = fmaf(pw, ev[e], o[e]);
-                    }
-                }
-                if (i < p.T) {
-#pragma unroll
-                    for (int g = 0; g < 4; g++) {
-                        uint4 u;
-                        u.x = pack_h2(o[8 * g] * inv, o[8 * g + 1] * inv); u.y = pack_h2(o[8 * g + 2] * inv, o[8 * g + 3] * inv);
-                        u.z = pack_h2(o[8 * g + 4] * inv, o[8 * g + 5] * inv); u.w = pack_h2(o[8 * g + 6] * inv, o[8 * g + 7] * inv);
-                        obase[(size_t)(c0 / 8 + g) * p.T + i] = u;
-                    }
-                }
-            }
-            }  // KS == 1
         }
+        // ---- park this CTA's partial rows in its own shared memory (the K/V stages, free once both warpgroups are done):
+        //      [27 float4][128 rows]: slots 0..23 unnormalised P.V (96 channels), 24 = (m, l, prel0, prel1), 25 = prel2..5, 26 = prel6..8
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        float* partf = reinterpret_cast<float*>(sK);
+#pragma unroll
+        for (int e = 0; e < DK / 2; e += 2) {
+            const int hr = (e >> 1) & 1, row = r0 + 8 * hr, ch = 8 * (e >> 2) + cq;
+            *reinterpret_cast<float2*>(&partf[((size_t)(ch >> 2) * 128 + row) * 4 + (ch & 3)]) = make_float2(o[e], o[e + 1]);
+        }
+        __syncwarp();  // sPrel entries of this warp's rows were written by the lanes of their quads
+        if ((t & 3) == 0) {
+            float4* part = reinterpret_cast<float4*>(sK);
+#pragma unroll
+            for (int hr = 0; hr < 2; hr++) {
+                const int row = r0 + 8 * hr;
+                float pr[NREL];
+#pragma unroll
+                for (int r = 0; r < NREL; r++) pr[r] = NT > 0 ? sPrel[r * 128 + row] : 0.f;
+                part[(size_t)24 * 128 + row] = make_float4(M[hr], L[hr], pr[0], pr[1]);
+                part[(size_t)25 * 128 + row] = make_float4(pr[2], pr[3], pr[4], pr[5]);
+                part[(size_t)26 * 128 + row] = make_float4(pr[6], pr[7], pr[8], 0.f);
+            }
+        }
+        if (stamp) prof[5] = gtimer();
     }
-    if (KS > 1 && NT_all > 0) {
+    if (NT_all > 0) {
         // ---- merge the key splits (every thread of every CTA of the cluster takes part in both barriers)
         if (stamp) prof[6] = gtimer();
         asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
         if (stamp) prof[7] = gtimer();
-        // CTA rk merges rows [rk * 128/KS, (rk + 1) * 128/KS); KS threads share a row (96/KS channels each), consecutive lanes take
+        // CTA rk merges rows [rk * 128/KS, (rk + 1) * 128/KS); KS threads share a row (96/KS channels each), consecutive threads take
         // consecutive rows (coalesced distributed-shared-memory reads)
-        if (warp >= 2) {
-            uint4* obase = p.att + ((size_t)b * H8 + (size_t)h * NG) * p.T;
-            if (KS == 4) attn_merge_rows<4, DK>(smem_u32(sK), sEv, rk, (warp - 2) * 32 + lane, q0, len, p.T, nrel, obase);
-            else attn_merge_rows<2, DK>(smem_u32(sK), sEv, rk, (warp - 2) * 32 + lane, q0, len, p.T, nrel, obase);
+        if (threadIdx.x < 128) {
+            if (KS == 4) attn_merge_rows<4, DK>(smem_u32(sK), sEv, rk, threadIdx.x, q0, len, p.T, nrel, obase);
+            else if (KS == 2) attn_merge_rows<2, DK>(smem_u32(sK), sEv, rk, threadIdx.x, q0, len, p.T, nrel, obase);
+            else attn_merge_rows<1, DK>(smem_u32(sK), sEv, rk, threadIdx.x, q0, len, p.T, nrel, obase);
         }
         if (stamp) prof[8] = gtimer();
         asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");  // peers are done reading this CTA's rows
     }
     if (stamp) prof[9] = gtimer();
-    fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
-    }
 }
 
-// MN-major no-swizzle B operand (v): which of LBO / SBO carries the stride between 8-key blocks (128 B) and which the stride
-// between 8-channel blocks (KT*16 B).  tests/cuda/tc_probe.cu (run_mn_probe) measures the convention on hardware.
-struct AttnMnConv { int lbo_is_kblock = 1; };
-
-inline size_t tc_flow_attn_smem(int DK, int KT) { return (size_t)DK * 128 * 2 + 4 * (size_t)DK * KT * 2 + 2 * (size_t)KT * 128 * 2 + 2 * 9 * (size_t)DK * 4 + 2 * 9 * 128 * 4 + 18 * 8 + 16; }
+inline size_t tc_flow_attn_smem(int DK, int KT) { return (size_t)DK * 128 * 2 + 4 * (size_t)DK * KT * 2 + 2 * 9 * (size_t)DK * 4 + 2 * 9 * 128 * 4 + 9 * 8 + 16; }
 
 inline void tc_flow_attn_init_device() {
     BV2_CUDA(cudaFuncSetAttribute(k_flow_attn<96, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
@@ -448,25 +368,22 @@ inline void tc_flow_attn_init_device() {
 
 // qkv16: 16-bit c8 tensor with C = 3H channels (Act.p reinterpreted); att16: 16-bit c8 tensor with C = H channels.
 inline void tc_flow_attn(const Act& qkv16, const Act& att16, const float* rel_k, const float* rel_v, const int* lens, int heads, int window,
-                         cudaStream_t st, AttnMnConv mn = AttnMnConv(), int num_sms = 148, int ks_override = 0, long long* prof = nullptr) {
+                         cudaStream_t st, int num_sms, int ks_override = 0, long long* prof = nullptr) {
     const int H = att16.C, dk = H / heads, KT = 128;
     BV2_CHECK(qkv16.C == 3 * H && dk == 96 && H % 8 == 0 && window <= 4 && qkv16.T == att16.T && qkv16.B == att16.B, "tc_flow_attn shapes (head dim 96, window <= 4)");
     AttnParams p{};
     p.qkv = reinterpret_cast<const uint4*>(qkv16.p); p.att = reinterpret_cast<uint4*>(att16.p);
     p.rel_k = rel_k; p.rel_v = rel_v; p.lens = lens;
     p.B = qkv16.B; p.T = qkv16.T; p.H = H; p.heads = heads; p.window = window; p.prof = prof;
-    p.idesc_qk = tc::make_idesc(1, KT);
-    p.idesc_pv = tc::make_idesc(1, dk) | (1u << 16);  // b_major = MN
-    const uint32_t kblk = 128u, nblk = (uint32_t)KT * 16u;
-    p.v_lbo = mn.lbo_is_kblock ? kblk : nblk; p.v_sbo = mn.lbo_is_kblock ? nblk : kblk;
+    p.v_lbo = 128u;                 // MN-major V: stride between 8-key core-matrix blocks (K direction)
+    p.v_sbo = (uint32_t)KT * 16u;   // ... and between 8-channel blocks (N direction)
     // key split: as many CTAs per query tile as keep the grid within one wave of the SMs and leave each CTA at least one key tile
     const int qtiles = cdiv(p.T, 128), ctas = qtiles * heads * p.B;
     int ks = 1;
     while (ks < 4 && 2 * ks <= qtiles && ctas * 2 * ks <= num_sms) ks *= 2;  // the merge is written for 2 or 4 splits
     if (ks_override > 0) ks = ks_override;
     p.ks = ks;
-    if (ks == 1) launch_pdl(k_flow_attn<96, 128>, dim3(qtiles, heads, p.B), dim3(192), tc_flow_attn_smem(dk, KT), st, p);
-    else launch_pdl_cluster(k_flow_attn<96, 128>, dim3(qtiles * ks, heads, p.B), dim3(192), tc_flow_attn_smem(dk, KT), st, ks, p);
+    launch_pdl_cluster(k_flow_attn<96, 128>, dim3(qtiles * ks, heads, p.B), dim3(288), tc_flow_attn_smem(dk, KT), st, ks, p);
 }
 
 }  // namespace bv2

@@ -1,11 +1,11 @@
-// tcgen05 (5th-gen tensor core) implicit-GEMM Conv1d on the c4 activation layout, fp32 accumulate in TMEM.
+// Hopper tensor-core (wgmma) implicit-GEMM Conv1d on the c4 activation layout, fp32 accumulators in a shared-memory image.
 // Replaces the 90 dilated MRF convolutions of the HiFi-GAN Generator (reference modules.py:296-309 via
 // models.py:546-552) = 96 % of the MACs of SynthesizerTrn.infer, the ups (models.py:543-545) and the flow convs.
 //
 // GEMM view of one CTA tile:  D[128 time steps, N = Cout] += sum_{tap j} sum_{ci}  A_j[t, ci] * W_j[ci, co]
 //   A_j[t, ci] = act(x[ci][t0 + t + j*dil - pad])  -- a time-shifted view of ONE staged activation tile.
 // A staged operand chunk is [KC/G channel groups][R = 128*MT + (K-1)*dil rows][16 bytes], i.e. the K-major / no-swizzle
-// UMMA canonical layout with SBO = 128 B (8 rows x 16 B) and LBO = R*16 B, so tap j is just the smem-descriptor start
+// wgmma canonical layout with SBO = 128 B (8 rows x 16 B) and LBO = R*16 B, so tap j is just the smem-descriptor start
 // address advanced by j*dil*16 bytes: the im2col matrix is never materialised and each activation byte is fetched from
 // HBM/L2 once per conv instead of K times.
 //
@@ -15,13 +15,12 @@
 //   F16 = 1  FP16 operands (kind::f16, K = 16 per MMA, G = 8 channels per group), fp32 activations in HBM as before: the
 //            prologue converts the staged fp32 c4 tile into a [KC/8][R][8 halves] image next to it.  FP16 has the same
 //            11-bit significand as TF32 (identical rounding error), twice the tensor-pipe rate, half the shared-memory
-//            operand bytes per MMA and half the L2->SM weight traffic -- the three things the round-1 ncu captures showed
-//            these kernels to be bound by.  Out-of-range values saturate (cvt.rn.satfinite) instead of becoming inf.
+//            operand bytes per MMA and half the L2->SM weight traffic.  Out-of-range values saturate (cvt.rn.satfinite) instead of becoming inf.
 //
-// Warp roles: warp 0 = TMA producer (cp.async.bulk, mbarrier complete_tx), warp 1 = TMEM allocator + single-thread
-// tcgen05.mma issuer, 4 warps = operand prologue (leaky-relu + operand conversion in smem, zero fill of the conv padding
-// rows, fence.proxy.async), 4 warps (the same ones in the one-tile kernel) = TMEM epilogue (accumulator init with
-// bias/residual via tcgen05.st, tail tcgen05.ld -> scale/mask -> coalesced 16-byte stores), +1 weight-producer warp.
+// Warp roles: warp 0 = TMA producer (cp.async.bulk, mbarrier complete_tx), one warpgroup at the end of the block = wgmma
+// issuer, 4 warps = operand prologue (leaky-relu + operand conversion in smem, zero fill of the conv padding
+// rows, fence.proxy.async), 4 warps (the same ones in the one-tile kernel) = epilogue (accumulator init with
+// bias/residual, tail -> scale/mask -> coalesced 16-byte stores, one thread per row of the accumulator image), +1 weight-producer warp.
 #pragma once
 #include <cstdlib>
 #include <cstring>
@@ -29,6 +28,7 @@
 #include <vector>
 #include <cuda_fp16.h>
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace bv2 {
 
@@ -95,14 +95,14 @@ inline int tune_env(const char* name, int dflt) {
 }
 
 // w: [Cout][Cin][K] fp32 (weight-norm already folded)
-// nt = N tile (0: largest divisor of Cout that is a multiple of 16 and <= 256)
+// nt = N tile (0: largest divisor of Cout that is a multiple of 16 and <= 128: a 128-column fp32 accumulator image is 66 KB of shared memory)
 // kc = K chunk (channels per pipeline stage)
 // fill = false: only the sizes / layout fields are computed and an all-zero image of the right size is handed to `up` (the engine's
 // measuring pass and bv2_load_packed, where the image comes from a file)
 inline TcConvW tc_pack_weights(std::function<float*(const std::vector<float>&)>& up, const std::vector<float>& w, int Cout, int Cin, int K, int nt = 0,
                                int f16 = 0, int kc = 0, bool fill = true) {
     TcConvW t; t.Cin = Cin; t.Cout = Cout; t.K = K; t.f16 = f16;
-    if (!nt) { nt = std::min(Cout, 256); while (Cout % nt || nt % 16) nt -= 16; }
+    if (!nt) { nt = std::min(Cout, 128); while (Cout % nt || nt % 16) nt -= 16; }
     kc = tune_env("BV2_TC_KC", kc);
     if (!kc) kc = 32;
     t.KC = Cin >= kc ? kc : Cin;
@@ -137,7 +137,7 @@ inline TcConvW tc_pack_weights(std::function<float*(const std::vector<float>&)>&
 // -> an ordinary conv over input-rate time with Kp taps (union of the per-phase offsets), N = u*Cout columns ordered
 // (r, co), structural zeros where a phase does not use a tap.  wT: [Cin][Cout][K] (weight-norm folded).
 inline TcConvW tc_pack_upsample(std::function<float*(const std::vector<float>&)>& up, const std::vector<float>& wT, int Cin, int Cout, int K, int u,
-                                int kc = 0, int f16 = 0, bool fill = true, int nt_max = 256) {
+                                int kc = 0, int f16 = 0, bool fill = true, int nt_max = 128) {
     const int p = (K - u) / 2, taps = K / u;
     int omin = 1 << 30, omax = -(1 << 30);
     for (int r = 0; r < u; r++)
@@ -163,7 +163,7 @@ struct TcParams {
     int Cin_total, cin_off, Cout_total, cout_off, res_C_total, res_c_off, bias_b_stride;
     int nt;           // columns per N tile
     int T, B, K, dil, pad, KC, nchunks, R, nws, nas, MT;
-    uint32_t a_stage_bytes, a_op_off, w_stage_bytes, tmem_cols, idesc;
+    uint32_t a_stage_bytes, a_op_off, w_stage_bytes, acc_cols;  // acc_cols: columns of the accumulator image
     float in_slope, out_scale;
     int accumulate, relu, res_mode, in_mask, out_mask, ups_u, ups_cout;
     int out_tf32, skip_xform, in_f16, out_f16, gate;
@@ -188,33 +188,30 @@ __device__ int g_tc_err_dev = 0;
 __device__ int* g_tc_err_flag = nullptr;
 
 namespace tc {
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* v) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-                 ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-                   "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]) : "memory");
+// Accumulators live in shared memory, in front of every tensor-core kernel's own buffers: an fp32 image [column][ACC_TS rows] of the
+// 128-row tile, addressed like a tensor-memory column/lane pair (taddr = row << 16 | column; the kernels' accumulator base is 0).
+// The MMA warpgroup streams one 64-row x <= 64-column slice of it through registers per weight stage (wg_mma); the epilogue threads
+// own one row each and read / write whole runs of columns.  ACC_TS = 132: the stride keeps both access patterns free of bank
+// conflicts (a warp's wgmma fragment touches rows r..r+7 of columns c, c+2, c+4, c+6: banks 8k + r).
+constexpr uint32_t ACC_TS = 132;
+__host__ __device__ constexpr uint32_t acc_img_bytes(uint32_t cols) { return (cols * ACC_TS * 4u + 1023u) & ~1023u; }
+extern __shared__ __align__(1024) uint8_t bv2_dyn_smem[];
+__device__ __forceinline__ float* acc_ptr(uint32_t taddr) {
+    return reinterpret_cast<float*>(bv2_dyn_smem) + (size_t)(taddr & 0xffffu) * ACC_TS + (taddr >> 16);
 }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* v) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-                 ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]),
-                   "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]),
-                   "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31]) : "memory");
+// 32x32b-style accesses: lane i of the calling warp takes row (taddr >> 16) + i, columns (taddr & 0xffff) + 0 .. n-1
+template <int N>
+__device__ __forceinline__ void acc_st(uint32_t taddr, const uint32_t* v) {
+    float* d = acc_ptr(taddr) + (threadIdx.x & 31);
+#pragma unroll
+    for (int i = 0; i < N; i++) d[i * ACC_TS] = __uint_as_float(v[i]);
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* v) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-                   "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-                 : "r"(taddr));
+template <int N>
+__device__ __forceinline__ void acc_ld(uint32_t taddr, uint32_t* v) {
+    const float* d = acc_ptr(taddr) + (threadIdx.x & 31);
+#pragma unroll
+    for (int i = 0; i < N; i++) v[i] = __float_as_uint(d[i * ACC_TS]);
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* v) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-                   "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]),
-                   "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]),
-                   "=r"(v[30]), "=r"(v[31])
-                 : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -251,13 +248,10 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
                  : "=r"(done) : "r"(bar), "r"(parity), "r"(1000000u) : "memory");
     if (!done) mbar_wait_slow(bar, parity);
 }
-// Bounded wait for the MMA-issuer warps, written as ONE asm block (no C++ control flow on a per-thread result, no call).
-// Why: ptxas keeps the issuer's descriptors / loop state in uniform registers and updates them with UIADD3 only while the
-// surrounding code is provably warp-uniform and free of calls (uniform registers do not survive a call).  mbar_wait() above
-// branches on a per-thread predicate into a noinline function with printf: every value that is live across it is demoted to
-// vector registers and each UTCHMMA then needs an ELECT + 5x R2UR.BROADCAST chain that re-uses one uniform-register set --
-// measured 180-570 cycles per MMA in k_g2_conv against the 64-cycle tensor time of an N = 128 MMA (profiles/r02_g2_issue.md).
-// Same timeout protocol as mbar_wait_slow (error flags raised, wait abandoned), minus the printf.
+// Bounded wait for the MMA warpgroups and the weight producers, written as ONE asm block (no C++ control flow on a per-thread
+// result, no call): a call inside the MMA loop would make ptxas serialise the wgmma pipeline across it (C7510) and demote the
+// loop's descriptor state from uniform registers.  Same timeout protocol as mbar_wait_slow (error flags raised, wait abandoned),
+// minus the printf.
 __device__ __forceinline__ void mbar_wait_u(uint32_t bar, uint32_t parity) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t.reg .u32 n, e;\n\t.reg .u64 t0, t1;\n\t"
@@ -296,71 +290,61 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// One lane of a fully converged warp.  The MMA issuer runs its loops with ALL 32 lanes (descriptors and loop state stay in uniform
-// registers) and only the tcgen05.mma / tcgen05.commit are guarded by this: issuing from inside an `if (lane == 0)` region makes
-// nvcc treat every operand as divergent and wrap each UTCHMMA in an ELECT + 5x R2UR.BROADCAST + BRA.U.ANY waterfall loop
-// (measured in round 2: ~185 cycles per MMA regardless of its size, 3x the 64-cycle MMA at N = 128).
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-// tcgen05.mma / tcgen05.commit with the lane election inside the asm block (statement stays in warp-uniform control flow)
-template <int F16>
-__device__ __forceinline__ void umma_el(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    if (F16)
-        asm volatile("{\n\t.reg .pred p, q;\n\tsetp.ne.b32 p, %4, 0;\n\telect.sync _|q, 0xffffffff;\n\t@q tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                     ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-    else
-        asm volatile("{\n\t.reg .pred p, q;\n\tsetp.ne.b32 p, %4, 0;\n\telect.sync _|q, 0xffffffff;\n\t@q tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-                     ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit_el(uint32_t bar) {
-    asm volatile("{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\t@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// K-major, SWIZZLE_NONE shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start>>4 [0,14), LBO>>4 [16,30),
-// SBO>>4 [32,46), version=1 [46,48), layout_type=0 [61,64)
+// K-major, no-swizzle shared-memory matrix descriptor (wgmma): start>>4 [0,14), LBO>>4 [16,30) = stride between core matrices along K,
+// SBO>>4 [32,46) = stride between 8-row core-matrix groups along M / N, layout type 0 (no swizzle) [62,64)
 __device__ __forceinline__ uint64_t make_desc(uint32_t addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    return (uint64_t)((addr & 0x3ffffu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) | (1ull << 46);
+    return (uint64_t)((addr & 0x3ffffu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32);
 }
-template <int F16>
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    if (F16)
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                     ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-    else
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-                     ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-template <int F16>
-__device__ __forceinline__ void umma_e(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    umma_el<F16>(tmem_d, adesc, bdesc, idesc, accumulate);
-}
-__device__ __forceinline__ void umma_commit_e(uint32_t bar) { umma_commit_el(bar); }
-// nk accumulating k-steps on one accumulator, unrolled for the common counts: a rolled loop re-uses one uniform-register set for the
-// descriptors and serialises every UTCHMMA behind the R2UR round trip of its predecessor (~190 cycles per MMA of any size, round 2)
-template <int F16, int NK>
-__device__ __forceinline__ void umma_ksteps_n(uint32_t d, uint64_t ad, uint64_t bd, uint64_t a_kstep, uint64_t b_kstep, uint32_t idesc, uint32_t acc_first) {
+// One 64-row x NC-column slice of the accumulator: image -> registers (or zeros), nk MMAs, registers -> image.
+template <int F16, int NC>
+__device__ __forceinline__ void wg_slice(float* img, uint64_t ad, uint64_t bd, uint64_t a_kstep, uint64_t b_kstep, int nk, uint32_t acc) {
+    float c[NC / 2];
+    const int cq = 2 * (threadIdx.x & 3);
 #pragma unroll
-    for (int kk = 0; kk < NK; kk++) umma_e<F16>(d, ad + kk * a_kstep, bd + kk * b_kstep, idesc, kk ? 1u : acc_first);
+    for (int i = 0; i < NC / 8; i++) {
+        const float* q = img + (size_t)(8 * i + cq) * ACC_TS;
+        c[4 * i] = acc ? q[0] : 0.f; c[4 * i + 1] = acc ? q[ACC_TS] : 0.f; c[4 * i + 2] = acc ? q[8] : 0.f; c[4 * i + 3] = acc ? q[ACC_TS + 8] : 0.f;
+    }
+    wgmma_fence();
+    for (int kk = 0; kk < nk; kk++) Wgmma<F16, NC>::mma(c, ad + (uint64_t)kk * a_kstep, bd + (uint64_t)kk * b_kstep);
+    wgmma_commit();
+    wgmma_wait0();
+#pragma unroll
+    for (int i = 0; i < NC / 8; i++) {
+        float* q = img + (size_t)(8 * i + cq) * ACC_TS;
+        q[0] = c[4 * i]; q[ACC_TS] = c[4 * i + 1]; q[8] = c[4 * i + 2]; q[ACC_TS + 8] = c[4 * i + 3];
+    }
 }
+// D[128 rows x n columns at accumulator column d] (+)= sum_kk A(ad + kk*a_kstep) . B(bd + kk*b_kstep), run by all 128 threads of the
+// MMA warpgroup.  M = 128 is two 64-row wgmma slices (A advanced by 8 SBO strides), N in slices of 64 / 32 / 16 columns (B advanced by
+// n/8 SBO strides).  acc = 0: the accumulator starts from zero.
 template <int F16>
-__device__ __forceinline__ void umma_ksteps(uint32_t d, uint64_t ad, uint64_t bd, uint64_t a_kstep, uint64_t b_kstep, uint32_t idesc, int nk, uint32_t acc_first) {
-    // at most three alternatives: with four or more the compiler builds a jump table (BRX on a vector register) and ptxas then treats
-    // everything after it as divergent, which takes the descriptors out of the uniform datapath (see mbar_wait_u)
-    if (nk == 2) umma_ksteps_n<F16, 2>(d, ad, bd, a_kstep, b_kstep, idesc, acc_first);
-    else if (nk == 4) umma_ksteps_n<F16, 4>(d, ad, bd, a_kstep, b_kstep, idesc, acc_first);
-    else
-        for (int kk = 0; kk < nk; kk++, ad += a_kstep, bd += b_kstep) umma_e<F16>(d, ad, bd, idesc, kk ? 1u : acc_first);
+__device__ __forceinline__ void wg_mma(uint32_t d, uint64_t ad, uint64_t bd, uint64_t a_kstep, uint64_t b_kstep, int nk, int n, uint32_t acc) {
+    const int t = threadIdx.x & 127;
+    const uint64_t a_sbo = (ad >> 32) & 0x3fffu, b_sbo = (bd >> 32) & 0x3fffu;
+#pragma unroll 1
+    for (int h = 0; h < 2; h++) {
+        const uint64_t ah = ad + (uint64_t)(8 * h) * a_sbo;
+        float* img = acc_ptr(d) + 64 * h + 16 * (t >> 5) + ((t & 31) >> 2);
+#pragma unroll 1
+        for (int n0 = 0; n0 < n;) {
+            const uint64_t bn = bd + (uint64_t)(n0 >> 3) * b_sbo;
+            float* im = img + (size_t)n0 * ACC_TS;
+            if (n - n0 >= 64) { wg_slice<F16, 64>(im, ah, bn, a_kstep, b_kstep, nk, acc); n0 += 64; }
+            else if (n - n0 >= 32) { wg_slice<F16, 32>(im, ah, bn, a_kstep, b_kstep, nk, acc); n0 += 32; }
+            else { wg_slice<F16, 16>(im, ah, bn, a_kstep, b_kstep, nk, acc); n0 += 16; }
+        }
+    }
+}
+// Signal an mbarrier once every MMA the warpgroup issued so far has completed and its accumulator slices are back in shared memory
+// (named barrier 1 = the MMA warpgroup).
+__device__ __forceinline__ void wg_commit(uint32_t bar) {
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+    if ((threadIdx.x & 127) == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 // round-to-nearest (ties away) TF32 with two integer instructions: identical bits to cvt.rna.tf32.f32 for finite inputs,
-// but issued on the ALU pipe (round 1 ncu: the cvt saturated the XU pipe at 94-98 % in the operand prologue)
+// but issued on the ALU pipe instead of the XU pipe the cvt shares with the prologue's other conversions
 __device__ __forceinline__ float to_tf32(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u); }
 // two fp32 -> packed f16x2 (lo in bits [0,16)), round-to-nearest-even, saturating
 __device__ __forceinline__ uint32_t pack_h2(float lo, float hi) {
@@ -368,17 +352,12 @@ __device__ __forceinline__ uint32_t pack_h2(float lo, float hi) {
     asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
     return r;
 }
-__host__ __device__ __forceinline__ uint32_t make_idesc(int f16, int n, int m = 128) {
-    // c_format = F32 [4,6); a_format/b_format [7,10)/[10,13): 0 = F16, 2 = TF32; N>>3 [17,23); M>>4 [24,29)
-    const uint32_t fmt = f16 ? 0u : 2u;
-    return (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
 
 // Pre-load one 128-row x nt accumulator tile: bias (+ per-batch bias) (+/- residual) (+ previous output).
-// All global loads of a 32-column batch are issued before the first tcgen05.st (memory-level parallelism: the
+// All global loads of a 32-column batch are issued before the first image stores (memory-level parallelism: the
 // epilogue warps are the only threads touching residual/output tensors).
 // GEN = 1: generic epilogue (polyphase ConvTranspose scatter, per-batch bias, relu, 16-bit output); GEN = 0: plain conv
-// epilogue.  The plain instantiation is 10-20 % faster on the MRF convs (measured): these kernels run at their register caps.
+// epilogue.  The plain instantiation keeps the MRF convs (most of the launches) free of the generic tail's registers and branches.
 template <int NG, int GEN>
 __device__ __forceinline__ void acc_init_tile(const TcParams& p, uint32_t trow, int b, int t, int n0, int nt, int yb = -1, int coff = -1, bool skip_res = false) {
     const bool ok = t < p.T;
@@ -428,14 +407,13 @@ __device__ __forceinline__ void acc_init_tile(const TcParams& p, uint32_t trow, 
                     v[4 * g] = __float_as_uint(o[4 * h + g].x); v[4 * g + 1] = __float_as_uint(o[4 * h + g].y);
                     v[4 * g + 2] = __float_as_uint(o[4 * h + g].z); v[4 * g + 3] = __float_as_uint(o[4 * h + g].w);
                 }
-                tmem_st16(trow + (uint32_t)(col0 + 16 * h), v);
+                acc_st<16>(trow + (uint32_t)(col0 + 16 * h), v);
             }
         }
     }
-    tmem_wait_st();
 }
 
-// Drain one accumulator tile: TMEM -> [relu] -> scale/mask -> c4 global (16-byte stores, coalesced across a warp).
+// Drain one accumulator tile: the accumulator image -> [relu] -> scale/mask -> c4 global (16-byte stores, coalesced across a warp).
 template <int NG, int GEN>
 __device__ __forceinline__ void acc_tail_tile(const TcParams& p, uint32_t trow, int b, int t, int n0, int nt, int len, int yb = -1, int coff = -1) {
     const bool ok = t < p.T;
@@ -448,8 +426,7 @@ __device__ __forceinline__ void acc_tail_tile(const TcParams& p, uint32_t trow, 
     for (int col0 = 0; col0 < nt; col0 += 4 * NG) {
         uint32_t v[NG / 4][16];
 #pragma unroll
-        for (int h = 0; h < NG / 4; h++) if (col0 + 16 * h < nt) tmem_ld16(trow + (uint32_t)(col0 + 16 * h), v[h]);
-        tmem_wait_ld();
+        for (int h = 0; h < NG / 4; h++) if (col0 + 16 * h < nt) acc_ld<16>(trow + (uint32_t)(col0 + 16 * h), v[h]);
         if (!ok) continue;
 #pragma unroll
         for (int h = 0; h < NG / 4; h++) {
@@ -503,17 +480,16 @@ __device__ __forceinline__ void acc_tail_tile(const TcParams& p, uint32_t trow, 
 
 // Tail with a fused LayerNorm over the nt = Cout channels of each row (reference attentions.py:21-24 after the residual add of
 // attentions.py:114,118): the accumulator already holds bias + residual + conv (accumulator-init fusion), so the row statistics
-// are three cheap passes over TMEM (16 TB/s) instead of a separate kernel with an HBM round trip.
+// are three passes over the shared-memory accumulator image instead of a separate kernel with an HBM round trip.
 __device__ __forceinline__ void acc_tail_ln(const TcParams& p, uint32_t trow, int b, int t, int nt, int len, const float4* rs = nullptr) {
     // rs: this thread's row of the TMA-staged residual tile ([nt/4][128 rows] float4, already offset by the row); nullptr = the residual
-    // was pre-loaded into the accumulator.  x = acc + residual is re-formed in each pass (shared-memory reads are cheap, TMEM is not written).
+    // was pre-loaded into the accumulator.  x = acc + residual is re-formed in each pass (shared-memory reads are cheap, the accumulator image is not written).
     const bool ok = t < p.T;
     float4* ybp = reinterpret_cast<float4*>(p.y) + (size_t)b * (p.Cout_total / 4) * p.T;
     float s = 0.f;
     for (int c0 = 0; c0 < nt; c0 += 32) {
         uint32_t v[32];
-        tmem_ld32(trow + (uint32_t)c0, v);
-        tmem_wait_ld();
+        acc_ld<32>(trow + (uint32_t)c0, v);
         if (rs) {
 #pragma unroll
             for (int g = 0; g < 8; g++) {
@@ -529,8 +505,7 @@ __device__ __forceinline__ void acc_tail_ln(const TcParams& p, uint32_t trow, in
     float q = 0.f;
     for (int c0 = 0; c0 < nt; c0 += 32) {
         uint32_t v[32];
-        tmem_ld32(trow + (uint32_t)c0, v);
-        tmem_wait_ld();
+        acc_ld<32>(trow + (uint32_t)c0, v);
         if (rs) {
 #pragma unroll
             for (int g = 0; g < 8; g++) {
@@ -550,8 +525,7 @@ __device__ __forceinline__ void acc_tail_ln(const TcParams& p, uint32_t trow, in
     const float m = (p.out_mask && t >= len) ? 0.f : 1.f;
     for (int c0 = 0; c0 < nt; c0 += 16) {
         uint32_t v[16];
-        tmem_ld16(trow + (uint32_t)c0, v);
-        tmem_wait_ld();
+        acc_ld<16>(trow + (uint32_t)c0, v);
         if (!ok) continue;
 #pragma unroll
         for (int g = 0; g < 4; g++) {
@@ -630,12 +604,13 @@ __device__ __forceinline__ void xform16_stage(const float4* S, uint4* O, int ncg
 // One 128*MT-row tile per CTA.  grid: (M blocks of MT*128 time steps, N tiles, B [* heads])
 //
 // Accumulator-init fusion: before the first MMA the epilogue warps pre-load  bias (+ per-batch bias) (+/- residual)
-// (+ previous output when accumulating)  into the TMEM accumulator with tcgen05.st while the first TMA loads are in
-// flight; every MMA then accumulates, and the tail is only  TMEM -> [relu] -> scale/mask -> store.
+// (+ previous output when accumulating)  into the accumulator image while the first TMA loads are in
+// flight; every MMA then accumulates, and the tail is only  the accumulator image -> [relu] -> scale/mask -> store.
 template <int GEN, int F16>
-__global__ void __launch_bounds__(224, 4) k_tc_conv1d(TcParams p) {
+__global__ void __launch_bounds__(384, 1) k_tc_conv1d(TcParams p) {
     using namespace tc;
-    extern __shared__ __align__(1024) uint8_t smem[];
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + acc_img_bytes(p.acc_cols);  // behind the accumulator image
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int MT = p.MT;
     const int t0 = blockIdx.x * 128 * MT, n0 = blockIdx.y * p.nt, z = blockIdx.z;
@@ -653,7 +628,6 @@ __global__ void __launch_bounds__(224, 4) k_tc_conv1d(TcParams p) {
     auto BAR = [&](int i) { return bar0 + 8u * (uint32_t)i; };
     const int B_AFULL = 0, B_AREADY = NAS, B_AEMPTY = 2 * NAS, B_WFULL = 3 * NAS, B_WEMPTY = 3 * NAS + p.nws, B_ACC = 3 * NAS + 2 * p.nws,
               B_INIT = B_ACC + 1, B_RES = B_ACC + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + B_RES + 1);
 
     if (threadIdx.x == 0) {
         for (int i = 0; i < NAS; i++) { mbar_init(BAR(B_AFULL + i), 1); mbar_init(BAR(B_AREADY + i), 128); mbar_init(BAR(B_AEMPTY + i), 1); }
@@ -663,27 +637,19 @@ __global__ void __launch_bounds__(224, 4) k_tc_conv1d(TcParams p) {
         mbar_init(BAR(B_RES), 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(p.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    fence_before();
     __syncthreads();
-    fence_after();
-    const uint32_t tmem = __shfl_sync(0xffffffffu, *tmem_slot, 0);  // shfl: a warp-uniform value for ptxas (uniform registers in the MMA issuer)
-    // Programmatic dependent launch: everything above (barrier init, TMEM allocation) overlapped the tail of the previous kernel in
-    // the stream.  Roles that touch only static data do not wait for it: the weight producer fills its ring and, when the accumulator
-    // init is bias-only, the epilogue warps pre-load the accumulators while the upstream kernel is still running (timelines in
-    // profiles/r02g_flow_conv_timelines.log: the init cost 5-6 us AFTER the wait before).  Everybody else waits, then releases the
-    // dependents (releasing them before the wait let the whole rest of the stream become resident at once: measured slower).
+    const uint32_t acc0 = 0;  // accumulator image base (acc_ptr)
+    // Programmatic dependent launch: everything above (barrier init) overlapped the tail of the previous kernel in the stream.  Roles
+    // that touch only static data do not wait for it: the weight producer fills its ring and, when the accumulator init is bias-only,
+    // the epilogue warps pre-load the accumulators while the upstream kernel is still running.  Everybody else waits, then releases
+    // the dependents (releasing them before the wait would let the whole rest of the stream become resident at once).
     auto gtimer = [] { long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; };
     long long* prof = p.prof ? p.prof + ((size_t)(blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 8 : nullptr;
     if (prof && threadIdx.x == 0) prof[0] = gtimer();
     // LayerNorm tail with a TMA-staged residual (p.res_soff): the residual tile is copied into shared memory by the activation producer
     // right after the PDL wait and added by the tail, so the accumulator init is bias-only (static data, runs ahead of the wait) and the
-    // MMAs never wait for residual loads.  (Pre-loading the residual into the accumulator took 15 us of a 24 us conv_o + LN launch: 12
-    // dependent rounds of 4 float4 loads per thread AFTER the wait, with the MMA issuer parked on the init barrier,
-    // profiles/r02h_flow_conv_timelines_f16_ffn.log.)
+    // MMAs never wait for residual loads (pre-loading the residual into the accumulator means dependent rounds of float4 loads per
+    // thread AFTER the wait, with the MMA warpgroup parked on the init barrier).
     const bool res_smem = GEN && p.res_soff != 0;
     const bool bias_only = (!p.res_mode || res_smem) && !p.accumulate;
     const bool static_role = (warp == 6 && !p.w_mode) || (warp >= 2 && warp <= 5 && bias_only);
@@ -763,16 +729,15 @@ __global__ void __launch_bounds__(224, 4) k_tc_conv1d(TcParams p) {
                 if (++sw == nws_u) { sw = 0; ph ^= 1u; dst = dst0; }
             }
         }
-    } else if (warp == 1) {
-        {  // all 32 lanes run the issue loop convergently; uniform-register issue path: mbar_wait_u + in-asm election (see mbar_wait_u)
-            // ===== MMA issuer: per weight tile, MT x KC/(2G) tcgen05.mma (M=128, N=nt), always accumulating.
-            // Descriptors are advanced with 64-bit adds on the (addr >> 4) field: this single thread is the issue
-            // bottleneck for narrow N, so the loop body is kept to a handful of integer instructions.
+    } else if (warp >= 8) {
+        {  // the 128 threads of the MMA warpgroup run the issue loop together (wgmma is warpgroup-collective)
+            // ===== MMA issuer: per weight tile, MT x KC/(2G) wgmma (M=128, N=nt), always accumulating.
+            // Descriptors are advanced with 64-bit adds on the (addr >> 4) field: ring slot, parity and addresses are carried
+            // incrementally, so the loop body between two stages is a handful of integer instructions.
             const uint32_t a_lbo = (uint32_t)R * 16u, b_lbo = (uint32_t)nt * 16u;
             const uint64_t a_kstep = (uint64_t)(2u * (uint32_t)R), b_kstep = (uint64_t)(2u * (uint32_t)nt);  // two channel groups per MMA
             const int nk = p.KC / (2 * G);
             mbar_wait_u(BAR(B_INIT), 0);
-            fence_after();
             // ring slot / parity / descriptor state carried incrementally: no runtime division or multiply per stage (see tc_gen.cuh)
             const uint64_t a_stage16 = (uint64_t)(p.a_stage_bytes >> 4), w_stage16 = (uint64_t)(p.w_stage_bytes >> 4);
             const uint64_t a_desc_base = make_desc(smem_u32(sA) + p.a_op_off, a_lbo, 128u), b_desc_base = make_desc(smem_u32(sW), b_lbo, 128u);
@@ -782,32 +747,30 @@ __global__ void __launch_bounds__(224, 4) k_tc_conv1d(TcParams p) {
             uint64_t a_cur = a_desc_base, b_cur = b_desc_base;
             for (int c = 0; c < p.nchunks; c++) {
                 mbar_wait_u(bar_ar + 8u * sa, aph);
-                fence_after();
                 if (prof && c == 0 && lane == 0) prof[2] = gtimer();
                 uint64_t a_tap = a_cur;
                 for (int j = 0; j < p.K; j++, a_tap += (uint64_t)(uint32_t)p.dil) {
                     mbar_wait_u(bar_wf + 8u * sw, wph);
-                    fence_after();
                     for (int mt = 0; mt < MT; mt++)
-                        umma_ksteps<F16>(tmem + (uint32_t)(mt * nt), a_tap + (uint64_t)(uint32_t)(mt * 128), b_cur, a_kstep, b_kstep, p.idesc, nk, 1u);
-                    umma_commit_e(bar_we + 8u * sw);
+                        wg_mma<F16>(acc0 + (uint32_t)(mt * nt), a_tap + (uint64_t)(uint32_t)(mt * 128), b_cur, a_kstep, b_kstep, nk, nt, 1u);
+                    wg_commit(bar_we + 8u * sw);
                     b_cur += w_stage16;
                     if (++sw == nws_u) { sw = 0; wph ^= 1u; b_cur = b_desc_base; }
                 }
-                umma_commit_e(bar_ae + 8u * sa);
+                wg_commit(bar_ae + 8u * sa);
                 a_cur += a_stage16;
                 if (++sa == nas_u) { sa = 0; aph ^= 1u; a_cur = a_desc_base; }
             }
-            umma_commit_e(BAR(B_ACC));
+            wg_commit(BAR(B_ACC));
             if (prof && lane == 0) prof[3] = gtimer();
         }
+    } else if (warp == 1 || warp == 7) {  // idle (the MMA warpgroup starts at a warpgroup boundary)
     } else {
         const int tid2 = threadIdx.x - 64;
         const int q = warp & 3;
         // ===== accumulator init (overlaps the first TMA loads)
         for (int mt = 0; mt < MT; mt++)
-            acc_init_tile<4, GEN>(p, tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(mt * nt), b, t0 + mt * 128 + q * 32 + lane, n0, nt, yb, cout_off, res_smem);
-        fence_before();
+            acc_init_tile<4, GEN>(p, acc0 + ((uint32_t)(q * 32) << 16) + (uint32_t)(mt * nt), b, t0 + mt * 128 + q * 32 + lane, n0, nt, yb, cout_off, res_smem);
         mbar_arrive(BAR(B_INIT));
         if (prof && tid2 == 0) prof[4] = gtimer();
         if (bias_only) {  // the init above touched static data only; everything below reads / overwrites tensors of the upstream kernel
@@ -843,40 +806,35 @@ __global__ void __launch_bounds__(224, 4) k_tc_conv1d(TcParams p) {
         }
         // ===== tail
         mbar_wait(BAR(B_ACC), 0);
-        fence_after();
         if (prof && tid2 == 0) prof[5] = gtimer();
         if (GEN && p.ln_gamma) {
             const float4* rs = nullptr;
             if (res_smem) { mbar_wait(BAR(B_RES), 0); rs = reinterpret_cast<const float4*>(smem + p.res_soff) + (q * 32 + lane); }
-            // (a 255-register instantiation that kept the 192-column row in registers -- one tcgen05.ld round trip instead of 24 -- ran
-            //  11.1 us instead of 13.2 us per launch back to back but 1 us per layer SLOWER inside the flow: profiles/r02k_ab_ln_regs_weight_ring.jsonl)
-            acc_tail_ln(p, tmem + ((uint32_t)(q * 32) << 16), b, t0 + q * 32 + lane, nt, len, rs);
+            acc_tail_ln(p, acc0 + ((uint32_t)(q * 32) << 16), b, t0 + q * 32 + lane, nt, len, rs);
         } else {
             for (int mt = 0; mt < MT; mt++)
-                acc_tail_tile<4, GEN>(p, tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(mt * nt), b, t0 + mt * 128 + q * 32 + lane, n0, nt, len, yb, cout_off);
+                acc_tail_tile<4, GEN>(p, acc0 + ((uint32_t)(q * 32) << 16) + (uint32_t)(mt * nt), b, t0 + mt * 128 + q * 32 + lane, n0, nt, len, yb, cout_off);
         }
         if (prof && tid2 == 0) prof[6] = gtimer();
     }
-    fence_before();
     __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(p.tmem_cols) : "memory");
-    }
 }
 
 // ------------------------------------------------------------------------------------------------------------
 // Persistent variant for narrow layers (Cin <= 32: Generator stages 3/4 = 36 of the 90 MRF convs, the last ups).
 // Those launches have thousands of 128-row tiles with only K * Cin/(2G) tiny MMAs each, so the one-tile-per-CTA kernel
-// is bound by its per-tile latency chain (launch, TMEM alloc, barrier init, TMA round trip, tail).  Here each CTA
+// is bound by its per-tile latency chain (launch, accumulator setup, barrier init, TMA round trip, tail).  Here each CTA
 //   * keeps ALL weight taps resident in shared memory (<= 45 KB, loaded once),
 //   * walks tiles blockIdx.x, +gridDim.x, ... with a 3-deep TMA ring for the activation tiles (producer runs ahead),
-//   * double-buffers the TMEM accumulator: the epilogue warps pre-load tile i+1's accumulator (bias/residual) and
-//     drain tile i-1 while the MMA warp works on tile i.
-// 320 threads: warp 0 producer, warp 1 MMA issuer, warps 2-5 operand prologue, warps 6-9 accumulator init + tail.
-template <int GEN, int OCC, int F16>
-__global__ void __launch_bounds__(320, OCC) k_tc_conv1d_persist(TcParams p, int mtiles, int ntiles_total) {
+//   * double-buffers the accumulator image: the epilogue warps pre-load tile i+1's accumulator (bias/residual) and
+//     drain tile i-1 while the MMA warpgroup works on tile i.
+// 512 threads: warp 0 producer, warps 2-5 operand prologue, warps 6-9 accumulator init + tail, warps 12-15 MMA warpgroup
+// (warps 1, 10, 11 idle: the warpgroup starts at a warpgroup boundary).
+template <int GEN, int F16>
+__global__ void __launch_bounds__(512, 1) k_tc_conv1d_persist(TcParams p, int mtiles, int ntiles_total) {
     using namespace tc;
-    extern __shared__ __align__(1024) uint8_t smem[];
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + acc_img_bytes(p.acc_cols);  // behind the accumulator image
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nt = p.nt, NAS = p.nas, R = p.R;
     const int G = F16 ? 8 : 4, ncg = p.KC / G, ncg_in = p.KC / 4;
@@ -887,7 +845,6 @@ __global__ void __launch_bounds__(320, OCC) k_tc_conv1d_persist(TcParams p, int 
     const uint32_t bar0 = smem_u32(bars);
     auto BAR = [&](int i) { return bar0 + 8u * (uint32_t)i; };
     const int B_WFULL = 0, B_AFULL = 1, B_AREADY = 1 + NAS, B_AEMPTY = 1 + 2 * NAS, B_INIT = 1 + 3 * NAS, B_ACC = 3 + 3 * NAS;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + B_ACC + 2);
 
     if (threadIdx.x == 0) {
         mbar_init(BAR(B_WFULL), 1);
@@ -895,14 +852,8 @@ __global__ void __launch_bounds__(320, OCC) k_tc_conv1d_persist(TcParams p, int 
         for (int i = 0; i < 2; i++) { mbar_init(BAR(B_INIT + i), 128); mbar_init(BAR(B_ACC + i), 1); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(p.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    fence_before();
     __syncthreads();
-    fence_after();
-    const uint32_t tmem = __shfl_sync(0xffffffffu, *tmem_slot, 0);  // shfl: a warp-uniform value for ptxas (uniform registers in the MMA issuer)
+    const uint32_t acc0 = 0;  // accumulator image base (acc_ptr)
     const int n_mine = (ntiles_total - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;  // tiles of this CTA
 
     if (warp == 0) {
@@ -927,9 +878,9 @@ __global__ void __launch_bounds__(320, OCC) k_tc_conv1d_persist(TcParams p, int 
                 bulk_g2s(smem_u32(sA + (size_t)sa * p.a_stage_bytes) + ((uint32_t)lane * R + (uint32_t)r_lo) * 16u, src, row_bytes, BAR(B_AFULL + sa));
             }
         }
-    } else if (warp == 1) {
+    } else if (warp >= 12) {
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-        {  // all 32 lanes run the issue loop convergently; uniform-register issue path: mbar_wait_u + in-asm election (see mbar_wait_u)
+        {  // the 128 threads of the MMA warpgroup run the issue loop together (wgmma is warpgroup-collective)
             const uint32_t a_lbo = (uint32_t)R * 16u, b_lbo = (uint32_t)nt * 16u;
             const uint64_t a_kstep = (uint64_t)(2u * (uint32_t)R), b_kstep = (uint64_t)(2u * (uint32_t)nt);
             const uint64_t b_tap = (uint64_t)((uint32_t)ncg * nt);  // next tap's weight tile, in 16-byte units
@@ -940,18 +891,18 @@ __global__ void __launch_bounds__(320, OCC) k_tc_conv1d_persist(TcParams p, int 
                 const int sa = i % NAS, ab = i & 1;
                 mbar_wait_u(BAR(B_INIT + ab), (i >> 1) & 1);
                 mbar_wait_u(BAR(B_AREADY + sa), (i / NAS) & 1);
-                fence_after();
                 const uint64_t a_desc0 = make_desc(smem_u32(sA + (size_t)sa * p.a_stage_bytes) + p.a_op_off, a_lbo, 128u);
-                const uint32_t d = tmem + (uint32_t)(ab * nt);
+                const uint32_t d = acc0 + (uint32_t)(ab * nt);
                 uint64_t bd_tap = b_desc0;
                 for (int j = 0; j < p.K; j++, bd_tap += b_tap) {
                     uint64_t ad = a_desc0 + (uint64_t)(uint32_t)(j * p.dil), bd = bd_tap;
-                    umma_ksteps<F16>(d, ad, bd, a_kstep, b_kstep, p.idesc, nk, 1u);
+                    wg_mma<F16>(d, ad, bd, a_kstep, b_kstep, nk, nt, 1u);
                 }
-                umma_commit_e(BAR(B_AEMPTY + sa));
-                umma_commit_e(BAR(B_ACC + ab));
+                wg_commit(BAR(B_AEMPTY + sa));
+                wg_commit(BAR(B_ACC + ab));
             }
         }
+    } else if (warp == 1 || warp >= 10) {  // idle (the MMA warpgroup starts at a warpgroup boundary)
     } else if (warp < 6) {
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
         // ===== operand prologue
@@ -973,12 +924,11 @@ __global__ void __launch_bounds__(320, OCC) k_tc_conv1d_persist(TcParams p, int 
     } else {
         asm volatile("griddepcontrol.wait;" ::: "memory");
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-        // ===== accumulator init (tile i+1) and tail (tile i), double-buffered TMEM
+        // ===== accumulator init (tile i+1) and tail (tile i), double-buffered accumulator image
         const int q = warp & 3;
         auto init_tile = [&](int i) {
             const int tile = blockIdx.x + i * gridDim.x, b = tile / mtiles, t0 = (tile - b * mtiles) * 128;
-            acc_init_tile<4, GEN>(p, tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)((i & 1) * nt), b, t0 + q * 32 + lane, 0, nt);
-            fence_before();
+            acc_init_tile<4, GEN>(p, acc0 + ((uint32_t)(q * 32) << 16) + (uint32_t)((i & 1) * nt), b, t0 + q * 32 + lane, 0, nt);
             mbar_arrive(BAR(B_INIT + (i & 1)));
         };
         if (n_mine > 0) init_tile(0);
@@ -987,33 +937,26 @@ __global__ void __launch_bounds__(320, OCC) k_tc_conv1d_persist(TcParams p, int 
             const int tile = blockIdx.x + i * gridDim.x, b = tile / mtiles, t0 = (tile - b * mtiles) * 128;
             const int len = p.lens ? p.lens[b] : p.T;
             mbar_wait(BAR(B_ACC + (i & 1)), (i >> 1) & 1);
-            fence_after();
-            acc_tail_tile<4, GEN>(p, tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)((i & 1) * nt), b, t0 + q * 32 + lane, 0, nt, len);
-            fence_before();  // order this tile's tcgen05.ld before the next init's tcgen05.st on the same columns
+            acc_tail_tile<4, GEN>(p, acc0 + ((uint32_t)(q * 32) << 16) + (uint32_t)((i & 1) * nt), b, t0 + q * 32 + lane, 0, nt, len);
         }
     }
-    fence_before();
     __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(p.tmem_cols) : "memory");
-    }
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// Persistent variant with STREAMED weights for wide layers (Cin >= 64): the canonical Blackwell GEMM structure.
+// Persistent variant with STREAMED weights for wide layers (Cin >= 64).
 // Each CTA walks tiles of MT*128 rows (n-tile fastest, so CTAs that share an activation tile run together and hit L2);
 // the TMA producers run continuously over the flat (tile, chunk, tap) sequence, so the activation ring (NAS deep) and
-// the weight ring (nws deep) stay full across tile boundaries; the TMEM accumulator is double-buffered so the
-// epilogue warps pre-load tile i+1's accumulator and drain tile i-1 while the MMA warp is busy with tile i.
-// MT = 2 (256 rows per tile): every weight stage feeds two 128-row MMAs, which halves the L2->SM weight traffic per
-// output row -- with one 128-row tile per weight pass these layers stream their whole weight tensor (0.36-1.4 MB) per
-// tile and are bound by the ~42 B/clk/SM L2 path, not by the tensor pipe (round-1 ncu: tensor 16-21 %, DRAM 14-21 %).
-// 352 threads: warp 0 activation producer, warp 1 MMA issuer, warps 2-5 operand prologue, warps 6-9 accumulator init +
-// tail, warp 10 weight producer.
+// the weight ring (nws deep) stay full across tile boundaries; the accumulator image is double-buffered so the
+// epilogue warps pre-load tile i+1's accumulator and drain tile i-1 while the MMA warpgroup is busy with tile i.
+// The launcher uses MT = 1: two 128 x nt accumulator images already take up to 132 KB of shared memory.
+// 512 threads: warp 0 activation producer, warps 2-5 operand prologue, warps 6-9 accumulator init + tail, warp 10 weight
+// producer, warps 12-15 MMA warpgroup (warps 1 and 11 idle).
 template <int GEN, int F16>
-__global__ void __launch_bounds__(352, 1) k_tc_conv1d_pstream(TcParams p, int mtiles, int ntiles, int tiles_total) {
+__global__ void __launch_bounds__(512, 1) k_tc_conv1d_pstream(TcParams p, int mtiles, int ntiles, int tiles_total) {
     using namespace tc;
-    extern __shared__ __align__(1024) uint8_t smem[];
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + acc_img_bytes(p.acc_cols);  // behind the accumulator image
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nt = p.nt, NAS = p.nas, NWS = p.nws, R = p.R, NCH = p.nchunks, MT = p.MT;
     const int G = F16 ? 8 : 4, ncg = p.KC / G, ncg_in = p.KC / 4;
@@ -1024,7 +967,6 @@ __global__ void __launch_bounds__(352, 1) k_tc_conv1d_pstream(TcParams p, int mt
     auto BAR = [&](int i) { return bar0 + 8u * (uint32_t)i; };
     const int B_AFULL = 0, B_AREADY = NAS, B_AEMPTY = 2 * NAS, B_WFULL = 3 * NAS, B_WEMPTY = 3 * NAS + NWS, B_INIT = 3 * NAS + 2 * NWS,
               B_ACC = B_INIT + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + B_ACC + 2);
 
     if (threadIdx.x == 0) {
         for (int i = 0; i < NAS; i++) { mbar_init(BAR(B_AFULL + i), 1); mbar_init(BAR(B_AREADY + i), 128); mbar_init(BAR(B_AEMPTY + i), 1); }
@@ -1032,14 +974,8 @@ __global__ void __launch_bounds__(352, 1) k_tc_conv1d_pstream(TcParams p, int mt
         for (int i = 0; i < 2; i++) { mbar_init(BAR(B_INIT + i), 128); mbar_init(BAR(B_ACC + i), 1); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(p.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    fence_before();
     __syncthreads();
-    fence_after();
-    const uint32_t tmem = __shfl_sync(0xffffffffu, *tmem_slot, 0);  // shfl: a warp-uniform value for ptxas (uniform registers in the MMA issuer)
+    const uint32_t acc0 = 0;  // accumulator image base (acc_ptr)
     const int n_mine = (tiles_total - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
     // tile -> (batch, m tile, n tile); n tile fastest
     auto decode = [&](int i, int& b, int& t0, int& ntile) {
@@ -1098,9 +1034,9 @@ __global__ void __launch_bounds__(352, 1) k_tc_conv1d_pstream(TcParams p, int mt
                 }
             }
         }
-    } else if (warp == 1) {
+    } else if (warp >= 12) {
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-        {  // all 32 lanes run the issue loop convergently; uniform-register issue path: mbar_wait_u + in-asm election (see mbar_wait_u)
+        {  // the 128 threads of the MMA warpgroup run the issue loop together (wgmma is warpgroup-collective)
             const uint32_t a_lbo = (uint32_t)R * 16u, b_lbo = (uint32_t)nt * 16u;
             const uint64_t a_kstep = (uint64_t)(2u * (uint32_t)R), b_kstep = (uint64_t)(2u * (uint32_t)nt);
             const int nk = p.KC / (2 * G);
@@ -1113,28 +1049,26 @@ __global__ void __launch_bounds__(352, 1) k_tc_conv1d_pstream(TcParams p, int mt
             for (int i = 0; i < n_mine; i++) {
                 const int ab = i & 1;
                 mbar_wait_u(BAR(B_INIT + ab), (i >> 1) & 1);
-                fence_after();
-                const uint32_t d0 = tmem + (uint32_t)(ab * MT * nt);
+                const uint32_t d0 = acc0 + (uint32_t)(ab * MT * nt);
                 for (int c = 0; c < NCH; c++) {
                     mbar_wait_u(bar_ar + 8u * sa, aph);
-                    fence_after();
                     uint64_t a_tap = a_cur;
                     for (int j = 0; j < p.K; j++, a_tap += (uint64_t)(uint32_t)p.dil) {
                         mbar_wait_u(bar_wf + 8u * sw, wph);
-                        fence_after();
                         for (int mt = 0; mt < MT; mt++)
-                            umma_ksteps<F16>(d0 + (uint32_t)(mt * nt), a_tap + (uint64_t)(uint32_t)(mt * 128), b_cur, a_kstep, b_kstep, p.idesc, nk, 1u);
-                        umma_commit_e(bar_we + 8u * sw);
+                            wg_mma<F16>(d0 + (uint32_t)(mt * nt), a_tap + (uint64_t)(uint32_t)(mt * 128), b_cur, a_kstep, b_kstep, nk, nt, 1u);
+                        wg_commit(bar_we + 8u * sw);
                         b_cur += w_stage16;
                         if (++sw == nws_u) { sw = 0; wph ^= 1u; b_cur = b_desc_base; }
                     }
-                    umma_commit_e(bar_ae + 8u * sa);
+                    wg_commit(bar_ae + 8u * sa);
                     a_cur += a_stage16;
                     if (++sa == nas_u) { sa = 0; aph ^= 1u; a_cur = a_desc_base; }
                 }
-                umma_commit_e(BAR(B_ACC + ab));
+                wg_commit(BAR(B_ACC + ab));
             }
         }
+    } else if (warp == 1 || warp == 11) {  // idle (the MMA warpgroup starts at a warpgroup boundary)
     } else if (warp < 6) {
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
         // ===== operand prologue over the flat (tile, chunk) sequence
@@ -1158,15 +1092,14 @@ __global__ void __launch_bounds__(352, 1) k_tc_conv1d_pstream(TcParams p, int mt
     } else {
         asm volatile("griddepcontrol.wait;" ::: "memory");
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-        // ===== accumulator init (tile i+1) and tail (tile i), double-buffered TMEM
+        // ===== accumulator init (tile i+1) and tail (tile i), double-buffered accumulator image
         const int q = warp & 3;
         auto init_tile = [&](int i) {
             int b, t0, ntile;
             decode(i, b, t0, ntile);
             const int n0 = ntile * nt;
             for (int mt = 0; mt < MT; mt++)
-                acc_init_tile<8, GEN>(p, tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(((i & 1) * MT + mt) * nt), b, t0 + mt * 128 + q * 32 + lane, n0, nt);
-            fence_before();
+                acc_init_tile<8, GEN>(p, acc0 + ((uint32_t)(q * 32) << 16) + (uint32_t)(((i & 1) * MT + mt) * nt), b, t0 + mt * 128 + q * 32 + lane, n0, nt);
             mbar_arrive(BAR(B_INIT + (i & 1)));
         };
         if (n_mine > 0) init_tile(0);
@@ -1177,262 +1110,11 @@ __global__ void __launch_bounds__(352, 1) k_tc_conv1d_pstream(TcParams p, int mt
             const int n0 = ntile * nt;
             const int len = p.lens ? p.lens[b] : p.T;
             mbar_wait(BAR(B_ACC + (i & 1)), (i >> 1) & 1);
-            fence_after();
             for (int mt = 0; mt < MT; mt++)
-                acc_tail_tile<8, GEN>(p, tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(((i & 1) * MT + mt) * nt), b, t0 + mt * 128 + q * 32 + lane, n0, nt, len);
-            fence_before();  // order this tile's tcgen05.ld before the next init's tcgen05.st on the same columns
+                acc_tail_tile<8, GEN>(p, acc0 + ((uint32_t)(q * 32) << 16) + (uint32_t)(((i & 1) * MT + mt) * nt), b, t0 + mt * 128 + q * 32 + lane, n0, nt, len);
         }
     }
-    fence_before();
     __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(p.tmem_cols) : "memory");
-    }
-}
-
-// ------------------------------------------------------------------------------------------------------------
-// Persistent fused ResBlock pair (reference modules.py:296-309):  y = conv2(lrelu(conv1(lrelu(x)))) + x  [(+ y_old) * scale]
-// conv1: K taps, dilation d;  conv2: K taps, dilation 1;  C <= 32 channels in and out.  One tile = TO = 128-(K-1) output
-// rows: conv1 accumulates 128 rows in TMEM (D1), the epilogue warps turn D1 into the A-operand image XT[C/G][128+K-1][16 B]
-// in SHARED memory (zero outside the sequence = conv2's padding), conv2 runs straight from XT through tap-shifted
-// descriptors into a second accumulator (D2) that was pre-loaded with bias2 + residual.  The intermediate never touches
-// HBM: 5 activation round trips per pair become ~2.5 and two launches become one.  Both weight tensors stay resident in
-// shared memory; each CTA walks tiles g = blockIdx.x, +gridDim.x, ... and software-pipelines them across the roles:
-//   warp 0      TMA producer: x tile i+2 while ...
-//   warps 2-5   operand prologue (lrelu + operand conversion) of x tile i+1
-//   warp 1      MMA: conv1(tile i+1) into D1[(i+1)&1], then conv2(tile i) from XT[i&1] into D2[i&1]
-//   warps 6-9   D2 init (bias2 + residual [+ y_old]) of tile i+1, D1 -> XT of tile i+1, tail (D2 -> HBM) of tile i
-// D1, D2 and XT are double-buffered, so conv2 of a tile overlaps conv1 of the next and both overlap the epilogues.
-struct TcPairPParams {
-    const float* x; float* y; const float* w1; const float* w2; const float* b1; const float* b2;
-    int C, T, B, K, dil, R1, RT, TO, nas, tiles_per_b, total_tiles;
-    uint32_t a_stage_bytes, a_op_off, w_bytes, xt_bytes, tmem_cols, idesc;
-    float out_scale; int accumulate;
-};
-
-template <int F16>
-__global__ void __launch_bounds__(320, 2) k_tc_pair_persist(TcPairPParams p) {
-    using namespace tc;
-    extern __shared__ __align__(1024) uint8_t smem[];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int C = p.C, NAS = p.nas, R = p.R1, RT = p.RT;
-    const int G = F16 ? 8 : 4, ncg = C / G, ncg_in = C / 4;
-    const int p2 = (p.K - 1) / 2, p1 = p2 * p.dil;
-    uint8_t* sW1 = smem;
-    uint8_t* sW2 = sW1 + p.w_bytes;
-    uint8_t* sA = sW2 + p.w_bytes;
-    uint8_t* sXT = sA + (size_t)NAS * p.a_stage_bytes;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sXT + 2 * (size_t)p.xt_bytes);
-    const uint32_t bar0 = smem_u32(bars);
-    auto BAR = [&](int i) { return bar0 + 8u * (uint32_t)i; };
-    const int B_AFULL = 0, B_AREADY = NAS, B_AEMPTY = 2 * NAS, B_W = 3 * NAS, B_D1FULL = B_W + 1, B_D1EMPTY = B_W + 3, B_XTFULL = B_W + 5,
-              B_D2FULL = B_W + 7, NBARS = B_W + 9;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + NBARS);
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < NAS; i++) { mbar_init(BAR(B_AFULL + i), 1); mbar_init(BAR(B_AREADY + i), 128); mbar_init(BAR(B_AEMPTY + i), 1); }
-        mbar_init(BAR(B_W), 1);
-        for (int i = 0; i < 2; i++) {
-            mbar_init(BAR(B_D1FULL + i), 1); mbar_init(BAR(B_D1EMPTY + i), 128); mbar_init(BAR(B_XTFULL + i), 128); mbar_init(BAR(B_D2FULL + i), 1);
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(p.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    fence_before();
-    __syncthreads();
-    fence_after();
-    const uint32_t tmem = __shfl_sync(0xffffffffu, *tmem_slot, 0);  // shfl: a warp-uniform value for ptxas (uniform registers in the MMA issuer)
-    const int ntl = (p.total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;  // tiles of this CTA
-    // tile i of this CTA -> (batch, first output row)
-    auto tile_bt = [&](int i, int& b, int& t0) {
-        const int g = (int)blockIdx.x + i * (int)gridDim.x;
-        b = g / p.tiles_per_b;
-        t0 = (g - b * p.tiles_per_b) * p.TO;
-    };
-
-    if (warp == 0) {
-        // resident weights: independent of the upstream kernel, so they load before the PDL wait
-        if (lane == 0) {
-            mbar_expect_tx(BAR(B_W), 2 * p.w_bytes);
-            bulk_g2s(smem_u32(sW1), p.w1, p.w_bytes, BAR(B_W));
-            bulk_g2s(smem_u32(sW2), p.w2, p.w_bytes, BAR(B_W));
-        }
-        asm volatile("griddepcontrol.wait;" ::: "memory");
-        asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-        for (int i = 0; i < ntl; i++) {
-            int b, t0; tile_bt(i, b, t0);
-            const int tx0 = t0 - p2 - p1;
-            const int r_lo = max(0, -tx0), r_hi = min(R, p.T - tx0);
-            const uint32_t row_bytes = (uint32_t)(r_hi - r_lo) * 16u;
-            const int sa = i % NAS;
-            if (lane == 0) {
-                mbar_wait(BAR(B_AEMPTY + sa), ((i / NAS) & 1) ^ 1);
-                mbar_expect_tx(BAR(B_AFULL + sa), row_bytes * ncg_in);
-            }
-            __syncwarp();
-            if (lane < ncg_in) {
-                const float* src = p.x + (((size_t)b * ncg_in + lane) * p.T + (tx0 + r_lo)) * 4;
-                bulk_g2s(smem_u32(sA + (size_t)sa * p.a_stage_bytes) + ((uint32_t)lane * R + (uint32_t)r_lo) * 16u, src, row_bytes, BAR(B_AFULL + sa));
-            }
-        }
-    } else if (warp == 1) {
-        asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-        {  // all 32 lanes run the issue loop convergently; uniform-register issue path: mbar_wait_u + in-asm election (see mbar_wait_u)
-            const uint32_t b_lbo = (uint32_t)C * 16u;
-            const uint64_t b_kstep = (uint64_t)(2u * (uint32_t)C);
-            const int nk = C / (2 * G);
-            const uint32_t tap_bytes = (uint32_t)C * (uint32_t)C * (F16 ? 2u : 4u);
-            mbar_wait_u(BAR(B_W), 0);
-            auto conv2 = [&](int i) {  // D2[i&1] += conv2(XT[i&1])
-                const int buf = i & 1;
-                mbar_wait_u(BAR(B_XTFULL + buf), (i >> 1) & 1);
-                fence_after();
-                const uint64_t xt0 = make_desc(smem_u32(sXT + (size_t)buf * p.xt_bytes), (uint32_t)RT * 16u, 128u);
-                const uint64_t a_kstep = (uint64_t)(2u * (uint32_t)RT);
-                const uint32_t d2 = tmem + (uint32_t)(2 * C + buf * C);
-                for (int j = 0; j < p.K; j++) {
-                    uint64_t ad = xt0 + (uint64_t)(uint32_t)j;
-                    uint64_t bd = make_desc(smem_u32(sW2) + (uint32_t)j * tap_bytes, b_lbo, 128u);
-                    umma_ksteps<F16>(d2, ad, bd, a_kstep, b_kstep, p.idesc, nk, 1u);
-                }
-                umma_commit_e(BAR(B_D2FULL + buf));
-            };
-            for (int i = 0; i < ntl; i++) {
-                const int sa = i % NAS, buf = i & 1;
-                mbar_wait_u(BAR(B_AREADY + sa), (i / NAS) & 1);
-                mbar_wait_u(BAR(B_D1EMPTY + buf), ((i >> 1) & 1) ^ 1);
-                fence_after();
-                const uint64_t a0 = make_desc(smem_u32(sA + (size_t)sa * p.a_stage_bytes) + p.a_op_off, (uint32_t)R * 16u, 128u);
-                const uint64_t a_kstep = (uint64_t)(2u * (uint32_t)R);
-                const uint32_t d1 = tmem + (uint32_t)(buf * C);
-                for (int j = 0; j < p.K; j++) {
-                    uint64_t ad = a0 + (uint64_t)(uint32_t)(j * p.dil);
-                    uint64_t bd = make_desc(smem_u32(sW1) + (uint32_t)j * tap_bytes, b_lbo, 128u);
-                    umma_ksteps<F16>(d1, ad, bd, a_kstep, b_kstep, p.idesc, nk, j ? 1u : 0u);
-                }
-                umma_commit_e(BAR(B_AEMPTY + sa));
-                umma_commit_e(BAR(B_D1FULL + buf));
-                if (i > 0) conv2(i - 1);
-            }
-            if (ntl > 0) conv2(ntl - 1);
-        }
-    } else if (warp < 6) {
-        asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-        const int tid2 = threadIdx.x - 64;
-        for (int i = 0; i < ntl; i++) {
-            int b, t0; tile_bt(i, b, t0);
-            const int tx0 = t0 - p2 - p1;
-            const int r_lo = max(0, -tx0), r_hi = min(R, p.T - tx0);
-            const int sa = i % NAS;
-            mbar_wait(BAR(B_AFULL + sa), (i / NAS) & 1);
-            uint8_t* st = sA + (size_t)sa * p.a_stage_bytes;
-            if (F16) xform16_stage(reinterpret_cast<const float4*>(st), reinterpret_cast<uint4*>(st + p.a_op_off), ncg, R, r_lo, r_hi, 0.1f, tid2);
-            else xform_stage(reinterpret_cast<float4*>(st), ncg, R, r_lo, r_hi, 0.1f, tid2);
-            fence_async_smem();
-            mbar_arrive(BAR(B_AREADY + sa));
-        }
-    } else {
-        asm volatile("griddepcontrol.wait;" ::: "memory");
-        asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-        const int q = warp & 3, m = q * 32 + lane;
-        const uint32_t trow = tmem + ((uint32_t)(q * 32) << 16);
-        // rows 128..RT-1 of both XT buffers feed only discarded output rows; zero them once so they stay finite
-        if (m < p.K - 1)
-            for (int buf = 0; buf < 2; buf++) {
-                uint4* XT = reinterpret_cast<uint4*>(sXT + (size_t)buf * p.xt_bytes);
-                for (int cg = 0; cg < ncg; cg++) XT[(size_t)cg * RT + 128 + m] = make_uint4(0u, 0u, 0u, 0u);
-            }
-        auto tail = [&](int i) {  // D2[i&1] -> scale -> HBM
-            int b, t0; tile_bt(i, b, t0);
-            const int buf = i & 1, t_out = t0 + m;
-            const bool ok_out = m < p.TO && t_out < p.T;
-            float4* yb = reinterpret_cast<float4*>(p.y) + (size_t)b * ncg_in * p.T;
-            mbar_wait(BAR(B_D2FULL + buf), (i >> 1) & 1);
-            fence_after();
-            for (int col = 0; col < C; col += 16) {
-                uint32_t v[16];
-                tmem_ld16(trow + (uint32_t)(2 * C + buf * C + col), v);
-                tmem_wait_ld();
-                if (!ok_out) continue;
-#pragma unroll
-                for (int g = 0; g < 4; g++)
-                    yb[(size_t)((col >> 2) + g) * p.T + t_out] = make_float4(__uint_as_float(v[4 * g]) * p.out_scale, __uint_as_float(v[4 * g + 1]) * p.out_scale,
-                                                                             __uint_as_float(v[4 * g + 2]) * p.out_scale, __uint_as_float(v[4 * g + 3]) * p.out_scale);
-            }
-            fence_before();
-        };
-        for (int i = 0; i < ntl; i++) {
-            int b, t0; tile_bt(i, b, t0);
-            const int buf = i & 1, t_out = t0 + m;
-            const bool ok_out = m < p.TO && t_out < p.T;
-            const float4* xb = reinterpret_cast<const float4*>(p.x) + (size_t)b * ncg_in * p.T;
-            const float4* yb = reinterpret_cast<const float4*>(p.y) + (size_t)b * ncg_in * p.T;
-            // ---- D2[buf] = bias2 + x (+ y_old): its previous user (tile i-2) was drained by tail(i-2) in program order
-            for (int col = 0; col < C; col += 16) {
-                uint32_t v2[16];
-#pragma unroll
-                for (int g = 0; g < 4; g++) {
-                    const int cg = (col >> 2) + g;
-                    float4 o = *reinterpret_cast<const float4*>(p.b2 + cg * 4);
-                    if (ok_out) {
-                        const float4 r = xb[(size_t)cg * p.T + t_out];
-                        o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w;
-                        if (p.accumulate) { const float4 a = yb[(size_t)cg * p.T + t_out]; o.x += a.x; o.y += a.y; o.z += a.z; o.w += a.w; }
-                    }
-                    v2[4 * g] = __float_as_uint(o.x); v2[4 * g + 1] = __float_as_uint(o.y); v2[4 * g + 2] = __float_as_uint(o.z); v2[4 * g + 3] = __float_as_uint(o.w);
-                }
-                tmem_st16(trow + (uint32_t)(2 * C + buf * C + col), v2);
-            }
-            tmem_wait_st();
-            // ---- D1[buf] -> + bias1 -> lrelu -> operand type -> XT[buf]   (XT[buf]'s previous reader, conv2(i-2), finished before tail(i-2) returned)
-            const int t_xt = t0 - p2 + m;
-            const bool xt_in = t_xt >= 0 && t_xt < p.T;
-            mbar_wait(BAR(B_D1FULL + buf), (i >> 1) & 1);
-            fence_after();
-            for (int col = 0; col < C; col += 16) {
-                uint32_t v[16];
-                tmem_ld16(trow + (uint32_t)(buf * C + col), v);
-                tmem_wait_ld();
-                float f[16];
-#pragma unroll
-                for (int g = 0; g < 4; g++) {
-                    const float4 bb = *reinterpret_cast<const float4*>(p.b1 + col + 4 * g);
-                    f[4 * g] = xt_in ? lrelu(__uint_as_float(v[4 * g]) + bb.x, 0.1f) : 0.f;
-                    f[4 * g + 1] = xt_in ? lrelu(__uint_as_float(v[4 * g + 1]) + bb.y, 0.1f) : 0.f;
-                    f[4 * g + 2] = xt_in ? lrelu(__uint_as_float(v[4 * g + 2]) + bb.z, 0.1f) : 0.f;
-                    f[4 * g + 3] = xt_in ? lrelu(__uint_as_float(v[4 * g + 3]) + bb.w, 0.1f) : 0.f;
-                }
-                if (F16) {
-                    uint4* XT = reinterpret_cast<uint4*>(sXT + (size_t)buf * p.xt_bytes);
-#pragma unroll
-                    for (int h = 0; h < 2; h++) {
-                        uint4 o;
-                        o.x = pack_h2(f[8 * h], f[8 * h + 1]); o.y = pack_h2(f[8 * h + 2], f[8 * h + 3]);
-                        o.z = pack_h2(f[8 * h + 4], f[8 * h + 5]); o.w = pack_h2(f[8 * h + 6], f[8 * h + 7]);
-                        XT[(size_t)((col >> 3) + h) * RT + m] = o;
-                    }
-                } else {
-                    float4* XT = reinterpret_cast<float4*>(sXT + (size_t)buf * p.xt_bytes);
-#pragma unroll
-                    for (int g = 0; g < 4; g++)
-                        XT[(size_t)((col >> 2) + g) * RT + m] = make_float4(to_tf32(f[4 * g]), to_tf32(f[4 * g + 1]), to_tf32(f[4 * g + 2]), to_tf32(f[4 * g + 3]));
-                }
-            }
-            fence_before();
-            mbar_arrive(BAR(B_D1EMPTY + buf));
-            fence_async_smem();
-            mbar_arrive(BAR(B_XTFULL + buf));
-            if (i > 0) tail(i - 1);
-        }
-        if (ntl > 0) tail(ntl - 1);
-    }
-    fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(p.tmem_cols) : "memory");
-    }
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1444,16 +1126,15 @@ inline void tc_clear_error() {
     const int z = 0;
     BV2_CUDA(cudaMemcpyToSymbol(g_tc_err_dev, &z, sizeof(z)));
 }
-// Returns the host view of this device's error flag (pinned, host-mapped; raised by a barrier timeout in any tcgen05 kernel).
+// Returns the host view of this device's error flag (pinned, host-mapped; raised by a barrier timeout in any wgmma kernel).
 inline int* tc_init_device() {
     const int mx = 227 * 1024;
 #define BV2_SMEM_ATTR(k) BV2_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, mx))
     BV2_SMEM_ATTR((k_tc_conv1d<0, 0>)); BV2_SMEM_ATTR((k_tc_conv1d<1, 0>)); BV2_SMEM_ATTR((k_tc_conv1d<0, 1>)); BV2_SMEM_ATTR((k_tc_conv1d<1, 1>));
-    BV2_SMEM_ATTR((k_tc_conv1d_persist<0, 2, 0>)); BV2_SMEM_ATTR((k_tc_conv1d_persist<1, 2, 0>));
-    BV2_SMEM_ATTR((k_tc_conv1d_persist<0, 2, 1>)); BV2_SMEM_ATTR((k_tc_conv1d_persist<1, 2, 1>));
+    BV2_SMEM_ATTR((k_tc_conv1d_persist<0, 0>)); BV2_SMEM_ATTR((k_tc_conv1d_persist<1, 0>));
+    BV2_SMEM_ATTR((k_tc_conv1d_persist<0, 1>)); BV2_SMEM_ATTR((k_tc_conv1d_persist<1, 1>));
     BV2_SMEM_ATTR((k_tc_conv1d_pstream<0, 0>)); BV2_SMEM_ATTR((k_tc_conv1d_pstream<1, 0>));
     BV2_SMEM_ATTR((k_tc_conv1d_pstream<0, 1>)); BV2_SMEM_ATTR((k_tc_conv1d_pstream<1, 1>));
-    BV2_SMEM_ATTR((k_tc_pair_persist<0>)); BV2_SMEM_ATTR((k_tc_pair_persist<1>));
 #undef BV2_SMEM_ATTR
     int* h = nullptr;
     BV2_CUDA(cudaHostAlloc(&h, sizeof(int), cudaHostAllocMapped));
@@ -1494,7 +1175,6 @@ inline void tc_conv1d(const TcConvW& w, const float* bias, const Act& x, const A
     if (e.out_f16) BV2_CHECK(F16 && !w.ups_u && e.cout_off % 8 == 0 && y.C % 8 == 0 && !e.res && !e.accumulate, "out_f16 epilogue");
     if (p.in_mask || p.out_mask) BV2_CHECK(e.lens != nullptr, "mask needs lens");
     BV2_CHECK(!(p.relu && (p.res_mode || p.accumulate)), "relu cannot be combined with residual/accumulate (accumulator-init fusion)");
-    p.idesc = tc::make_idesc(F16, nt);
     const bool generic = w.ups_u || e.bias_b || e.relu || e.out_f16 || e.ln_gamma || e.gate;
     const uint32_t esz = F16 ? 2u : 4u;
     p.w_stage_bytes = (uint32_t)(p.KC * nt) * esz;
@@ -1506,50 +1186,43 @@ inline void tc_conv1d(const TcConvW& w, const float* bias, const Act& x, const A
     set_rows(1);
     const long long nctas = (long long)cdiv(p.T, 128) * ntiles * p.B;
 
-    // ---- narrow layer with many tiles: persistent CTAs, resident weights, double-buffered TMEM
+    // ---- narrow layer with many tiles: persistent CTAs, resident weights, double-buffered accumulator image
     const size_t w_all = (size_t)p.K * p.KC * nt * esz;
     if (tune_env("BV2_TC_PERSIST", 1) && !e.skip_xform && !e.in_f16 && !e.out_f16 && !e.ln_gamma && !e.gate && p.nchunks == 1 && ntiles == 1 && w_all <= 64 * 1024 && nctas >= 2 * num_sms) {
         p.nas = 3;
         const size_t wb = (w_all + 127) & ~(size_t)127;
-        const size_t smem_p = wb + (size_t)p.nas * p.a_stage_bytes + (size_t)(3 * p.nas + 5) * 8 + 16;
-        uint32_t pc = 32; while ((int)pc < 2 * nt) pc <<= 1;
-        p.tmem_cols = pc;
-        // measured (round 1): 2 CTAs/SM with ~100 registers (no spills) beat 3 with 68 for the plain epilogue
-        const int per_sm = smem_p <= 110 * 1024 ? 2 : 1;
+        p.acc_cols = (uint32_t)(2 * nt);
+        const size_t smem_p = tc::acc_img_bytes(p.acc_cols) + wb + (size_t)p.nas * p.a_stage_bytes + (size_t)(3 * p.nas + 5) * 8 + 16;
+        const int per_sm = 1;  // 512 threads at > 64 registers: one CTA per SM
         const int mtiles = cdiv(p.T, 128);
         const int total = mtiles * p.B;
         const int grid_p = std::min(total, per_sm * num_sms);
-        if (generic) launch_pdl(F16 ? k_tc_conv1d_persist<1, 2, 1> : k_tc_conv1d_persist<1, 2, 0>, dim3(grid_p), dim3(320), smem_p, st, p, mtiles, total);
-        else launch_pdl(F16 ? k_tc_conv1d_persist<0, 2, 1> : k_tc_conv1d_persist<0, 2, 0>, dim3(grid_p), dim3(320), smem_p, st, p, mtiles, total);
+        if (generic) launch_pdl(F16 ? k_tc_conv1d_persist<1, 1> : k_tc_conv1d_persist<1, 0>, dim3(grid_p), dim3(512), smem_p, st, p, mtiles, total);
+        else launch_pdl(F16 ? k_tc_conv1d_persist<0, 1> : k_tc_conv1d_persist<0, 0>, dim3(grid_p), dim3(512), smem_p, st, p, mtiles, total);
         return;
     }
-    // ---- wide layer with at least one tile per SM: persistent CTAs, continuously streamed weights, double-buffered TMEM
-    if (tune_env("BV2_TC_PSTREAM", 1) && !e.skip_xform && !e.in_f16 && !e.ln_gamma && nctas >= num_sms && nt >= 64 && 2 * nt <= 512) {
-        // MT = 2 (256-row tiles) when both accumulator pairs fit TMEM and there are enough 256-row tiles to fill the SMs
-        int MT = (4 * nt <= 512 && (long long)cdiv(p.T, 256) * ntiles * p.B >= num_sms) ? 2 : 1;
-        MT = tune_env("BV2_PSTREAM_MT", MT);
-        if (4 * nt > 512) MT = 1;
+    // ---- wide layer with at least one tile per SM: persistent CTAs, continuously streamed weights, double-buffered accumulator image
+    // (only when two activation and two weight stages fit next to the double-buffered accumulator image; otherwise one tile per CTA)
+    if (tune_env("BV2_TC_PSTREAM", 1) && !e.skip_xform && !e.in_f16 && !e.ln_gamma && nctas >= num_sms && nt >= 64 &&
+        tc::acc_img_bytes((uint32_t)(2 * nt)) + 2ull * p.a_stage_bytes + 2ull * p.w_stage_bytes + 2048 <= 220 * 1024) {
+        // 128-row tiles: the double-buffered accumulator image (2 x nt columns) already takes up to 132 KB of shared memory
+        const int MT = 1;
         set_rows(MT);
-        const uint32_t big = 220 * 1024;
+        const uint32_t img = tc::acc_img_bytes((uint32_t)(2 * MT * nt));
+        const uint32_t big = 220 * 1024 - img;
         int nas2 = std::min(4, std::max(2, p.nchunks * 2));
         while (nas2 > 2 && (size_t)nas2 * p.a_stage_bytes + 3 * (size_t)p.w_stage_bytes + 2048 > big) nas2--;
-        if ((size_t)nas2 * p.a_stage_bytes + 2 * (size_t)p.w_stage_bytes + 2048 > big && MT == 2) {  // does not fit: fall back to 128-row tiles
-            MT = 1; set_rows(1);
-            nas2 = std::min(4, std::max(2, p.nchunks * 2));
-            while (nas2 > 2 && (size_t)nas2 * p.a_stage_bytes + 3 * (size_t)p.w_stage_bytes + 2048 > big) nas2--;
-        }
         int nws2 = (int)((big - (size_t)nas2 * p.a_stage_bytes - 2048) / p.w_stage_bytes);
         nws2 = std::max(2, std::min(nws2, 8));
         p.nas = nas2; p.nws = nws2;
-        uint32_t pc = 32; while ((int)pc < 2 * MT * nt) pc <<= 1;
-        p.tmem_cols = pc;
-        const size_t smem_s = (size_t)nas2 * p.a_stage_bytes + (size_t)nws2 * p.w_stage_bytes + (size_t)(3 * nas2 + 2 * nws2 + 4) * 8 + 16;
+        p.acc_cols = (uint32_t)(2 * MT * nt);
+        const size_t smem_s = img + (size_t)nas2 * p.a_stage_bytes + (size_t)nws2 * p.w_stage_bytes + (size_t)(3 * nas2 + 2 * nws2 + 4) * 8 + 16;
         BV2_CHECK(smem_s <= 227 * 1024, "tc_conv1d pstream shared memory");
         const int mtiles = cdiv(p.T, 128 * MT);
         const int total = mtiles * p.B * ntiles;
         const int grid_s = std::min(total, num_sms);
-        if (generic) launch_pdl(F16 ? k_tc_conv1d_pstream<1, 1> : k_tc_conv1d_pstream<1, 0>, dim3(grid_s), dim3(352), smem_s, st, p, mtiles, ntiles, total);
-        else launch_pdl(F16 ? k_tc_conv1d_pstream<0, 1> : k_tc_conv1d_pstream<0, 0>, dim3(grid_s), dim3(352), smem_s, st, p, mtiles, ntiles, total);
+        if (generic) launch_pdl(F16 ? k_tc_conv1d_pstream<1, 1> : k_tc_conv1d_pstream<1, 0>, dim3(grid_s), dim3(512), smem_s, st, p, mtiles, ntiles, total);
+        else launch_pdl(F16 ? k_tc_conv1d_pstream<0, 1> : k_tc_conv1d_pstream<0, 0>, dim3(grid_s), dim3(512), smem_s, st, p, mtiles, ntiles, total);
         return;
     }
     // ---- one tile per CTA.  Shared memory per CTA is capped (~48 KB) when there are more CTAs than SMs so that several
@@ -1560,25 +1233,25 @@ inline void tc_conv1d(const TcConvW& w, const float* bias, const Act& x, const A
     // LayerNorm tail with a residual, at most one CTA per SM (small batches: the launch is a latency chain, not a throughput problem):
     // the residual tile is staged in shared memory by TMA (nt/4 channel groups x 128 rows x 16 B) instead of being pre-loaded into the
     // accumulator; the rings shrink to make room (the weight ring never needs more stages than the conv has)
-    const bool res_smem = e.ln_gamma && p.res_mode == 1 && !p.accumulate && nctas <= num_sms && p.res_c_off % 4 == 0 && tune_env("BV2_LN_RES_SMEM", 1);
+    const bool res_smem = e.ln_gamma && p.res_mode == 1 && !p.accumulate && nctas <= num_sms && p.res_c_off % 4 == 0 && tune_env("BV2_LN_RES_SMEM", 1) &&
+                          tc::acc_img_bytes((uint32_t)nt) + (size_t)nt * 512u + 2ull * p.a_stage_bytes + 2ull * p.w_stage_bytes + 2048 <= 224 * 1024;
     const uint32_t res_bytes = res_smem ? (uint32_t)nt * 512u : 0u;
-    if (res_smem) budget = 224 * 1024 - res_bytes;
+    const uint32_t img = tc::acc_img_bytes((uint32_t)nt);
+    budget = std::min(budget, 224u * 1024u - img);
+    if (res_smem) budget = 224 * 1024 - img - res_bytes;
     int nas = std::min(3, std::max(2, p.nchunks));
     while (nas > 2 && (size_t)nas * p.a_stage_bytes + 4 * (size_t)p.w_stage_bytes + 1024 > budget) nas--;
     p.nas = nas;
     int nws = ((int)budget - nas * (int)p.a_stage_bytes - 1024) / (int)p.w_stage_bytes;
-    // (a ring as deep as the conv on small grids -- every weight stage of a 36-stage FFN conv_2 tile in flight ahead of the PDL wait -- measured
-    //  no gain: 14.2 -> 14.1 us per launch, profiles/r02k_ab_ln_regs_weight_ring.jsonl)
     p.nws = std::max(2, std::min(nws, tune_env("BV2_TC_NWS_MAX", 8)));
     p.nws = std::max(2, std::min(p.nws, p.nchunks * p.K));
-    uint32_t cols = 32; while ((int)cols < nt) cols <<= 1;
-    p.tmem_cols = cols;
-    size_t smem = (size_t)p.nas * p.a_stage_bytes + (size_t)p.nws * p.w_stage_bytes + (size_t)(3 * p.nas + 2 * p.nws + 3) * 8 + 16;
-    if (res_smem) { smem = (smem + 15) & ~(size_t)15; p.res_soff = (uint32_t)smem; smem += res_bytes; }
+    p.acc_cols = (uint32_t)nt;
+    size_t smem = img + (size_t)p.nas * p.a_stage_bytes + (size_t)p.nws * p.w_stage_bytes + (size_t)(3 * p.nas + 2 * p.nws + 3) * 8 + 16;
+    if (res_smem) { smem = (smem + 15) & ~(size_t)15; p.res_soff = (uint32_t)(smem - img); smem += res_bytes; }  // offset from the kernel's `smem` (behind the image)
     BV2_CHECK(smem <= 227 * 1024, "tc_conv1d shared memory");
     dim3 grid(cdiv(p.T, 128), ntiles, p.B);
-    if (generic) launch_pdl(F16 ? k_tc_conv1d<1, 1> : k_tc_conv1d<1, 0>, grid, dim3(224), smem, st, p);
-    else launch_pdl(F16 ? k_tc_conv1d<0, 1> : k_tc_conv1d<0, 0>, grid, dim3(224), smem, st, p);
+    if (generic) launch_pdl(F16 ? k_tc_conv1d<1, 1> : k_tc_conv1d<1, 0>, grid, dim3(384), smem, st, p);
+    else launch_pdl(F16 ? k_tc_conv1d<0, 1> : k_tc_conv1d<0, 0>, grid, dim3(384), smem, st, p);
 }
 
 // TF32 batched GEMMs on c4 operands (attention of the tf32 engine).
@@ -1588,19 +1261,18 @@ inline void tc_launch_simple(TcParams& p, int ntiles, int zdim, cudaStream_t st)
     p.a_stage_bytes = (uint32_t)(p.KC * p.R * 4); p.a_op_off = 0;
     p.w_stage_bytes = (uint32_t)(p.KC * p.nt * 4);
     const long long nctas = (long long)cdiv(p.T, 128) * ntiles * zdim;
-    const uint32_t budget = nctas > 148 ? 100 * 1024 : 200 * 1024;
+    const uint32_t img = tc::acc_img_bytes((uint32_t)p.nt);
+    const uint32_t budget = std::min<uint32_t>(nctas > 132 ? 100 * 1024 : 200 * 1024, 220 * 1024 - img);
     int nas = std::min(3, std::max(2, p.nchunks));
     while (nas > 2 && (size_t)nas * p.a_stage_bytes + 3 * (size_t)p.w_stage_bytes + 1024 > budget) nas--;
     p.nas = nas;
     int nws = ((int)budget - nas * (int)p.a_stage_bytes - 1024) / (int)p.w_stage_bytes;
     p.nws = std::max(2, std::min(nws, 8));
-    uint32_t cols = 32; while ((int)cols < p.nt) cols <<= 1;
-    p.tmem_cols = cols;
-    p.idesc = tc::make_idesc(0, p.nt);
-    const size_t smem = (size_t)p.nas * p.a_stage_bytes + (size_t)p.nws * p.w_stage_bytes + (size_t)(3 * p.nas + 2 * p.nws + 3) * 8 + 16;
+    p.acc_cols = (uint32_t)p.nt;
+    const size_t smem = img + (size_t)p.nas * p.a_stage_bytes + (size_t)p.nws * p.w_stage_bytes + (size_t)(3 * p.nas + 2 * p.nws + 3) * 8 + 16;
     BV2_CHECK(smem <= 227 * 1024, "tc gemm shared memory");
     dim3 grid(cdiv(p.T, 128), ntiles, zdim);
-    launch_pdl(k_tc_conv1d<0, 0>, grid, dim3(224), smem, st, p);
+    launch_pdl(k_tc_conv1d<0, 0>, grid, dim3(384), smem, st, p);
 }
 
 // S[z][keys][queries] (c4 over keys) = Q . K^T for every (batch, head): qkv c4 [B][3H/4][T][4], q pre-scaled.
@@ -1633,48 +1305,6 @@ inline void tc_attn_pv(const Act& P, const float* vt, int H, int heads, const Ac
     p.out_tf32 = 1;    // conv_o consumes it without a prologue
     BV2_CHECK(dk % 16 == 0 && dk <= 256 && P.C % 64 == 0 && P.B == att.B * heads && att.T == P.T, "tc_attn_pv shapes");
     tc_launch_simple(p, 1, P.B, st);
-}
-
-// Fused ResBlock pair launcher; returns false when the shapes do not fit (caller falls back to two launches).
-inline bool tc_pair_persist(const TcConvW& w1, const TcConvW& w2, const float* b1, const float* b2, const Act& x, const Act& y, int dil, float out_scale,
-                            int accumulate, cudaStream_t st, int num_sms) {
-    const int C = w1.Cin, F16 = w1.f16;
-    if (!(w1.Cout == C && w2.Cin == C && w2.Cout == C && w1.K == w2.K && w1.KC == C && w2.KC == C && w1.nt == C && w2.nt == C && w2.f16 == F16 && !w1.ups_u &&
-          C <= 32 && C % 16 == 0 && (w1.K & 1)))
-        return false;
-    const uint32_t esz = F16 ? 2u : 4u;
-    TcPairPParams p{};
-    p.x = x.p; p.y = y.p; p.w1 = w1.w; p.w2 = w2.w; p.b1 = b1; p.b2 = b2;
-    p.C = C; p.T = x.T; p.B = x.B; p.K = w1.K; p.dil = dil;
-    p.R1 = 128 + (p.K - 1) * dil; p.RT = 128 + p.K - 1; p.TO = 128 - (p.K - 1);
-    if (F16) { p.a_op_off = (uint32_t)(C * p.R1 * 4); p.a_stage_bytes = (uint32_t)(C * p.R1 * 6); }
-    else { p.a_op_off = 0; p.a_stage_bytes = (uint32_t)(C * p.R1 * 4); }
-    p.w_bytes = (uint32_t)(p.K * C * C) * esz; p.xt_bytes = (uint32_t)(C * p.RT) * esz;
-    p.tiles_per_b = cdiv(p.T, p.TO); p.total_tiles = p.tiles_per_b * p.B;
-    uint32_t cols = 32; while ((int)cols < 4 * C) cols <<= 1;
-    p.tmem_cols = cols;
-    p.idesc = tc::make_idesc(F16, C);
-    p.out_scale = out_scale; p.accumulate = accumulate;
-    static const int regs[2] = {[] { cudaFuncAttributes a{}; cudaFuncGetAttributes(&a, k_tc_pair_persist<0>); return a.numRegs; }(),
-                                [] { cudaFuncAttributes a{}; cudaFuncGetAttributes(&a, k_tc_pair_persist<1>); return a.numRegs; }()};
-    const int min_occ = tune_env("BV2_PPAIR_MINOCC", 2);
-    int occ = 0;
-    size_t smem = 0;
-    for (int nas = 3; nas >= 2; nas--) {  // prefer the 3-deep activation ring, drop to 2 if that buys a second resident CTA
-        p.nas = nas;
-        smem = 2 * (size_t)p.w_bytes + (size_t)nas * p.a_stage_bytes + 2 * (size_t)p.xt_bytes + (size_t)(3 * nas + 9) * 8 + 16;
-        if (smem > 227 * 1024) continue;
-        // resident CTAs per SM: shared memory (228 KB/SM, 1 KB reserved per CTA), registers (64K/SM), TMEM columns (512/SM)
-        occ = (int)((228 * 1024) / (smem + 1024));
-        occ = std::min(occ, 65536 / (320 * std::max(regs[F16], 1)));
-        occ = std::min(occ, (int)(512 / p.tmem_cols));
-        occ = std::min(occ, 4);
-        if (occ >= min_occ) break;
-    }
-    if (occ < min_occ) return false;  // one CTA per SM cannot hide the per-tile latency chain: the two-launch path is faster
-    const int grid = std::min(p.total_tiles, num_sms * occ);
-    launch_pdl(F16 ? k_tc_pair_persist<1> : k_tc_pair_persist<0>, dim3(grid), dim3(320), smem, st, p);
-    return true;
 }
 
 }  // namespace bv2

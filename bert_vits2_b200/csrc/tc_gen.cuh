@@ -11,18 +11,19 @@
 //     applies it once; the one other use, the residual `x + conv2(..)`, recovers x = a >= 0 ? a : 10 a  (lrelu is invertible);
 //     conv_post's lrelu(., 0.01) is a >= 0 ? a : 0.1 a.  CPU simulation of the f16 storage on the oracle: waveform RMS error
 //     7.7e-5 (f16 operands, fp32 activations) -> 1.0e-4 (f16 storage), bar 1e-3.
-//   * a [KC/8][R rows][16 B] window of such a tensor is the K-major no-swizzle UMMA operand tile: the TMA producer copies it
+//   * a [KC/8][R rows][16 B] window of such a tensor is the K-major no-swizzle wgmma operand tile: the TMA producer copies it
 //     straight into the ring (one cp.async.bulk per channel group), the MMA warp consumes it -- no prologue warps, 2 B of smem
 //     per element, and conv zero padding is the tensor's own zero halo (no per-tile fill, no predicates);
 //   * tap j of a dilated conv is the same staged tile with the descriptor start advanced by j*dil rows (as in tc_conv.cuh).
 //
-// One kernel, k_g2_conv: a CTA owns a super-tile of NG x MG m-tiles (128 rows each) x nt <= 128 columns, NG*MG*nt <= 512 TMEM
-// columns (the whole accumulator of the super-tile lives in TMEM), so each weight stage (chunk c, tap j) feeds MG*KC/16 MMAs:
-//   streamed weights (C >= 64): NG = 1, MG = 2..8 -- weights cross L2->SM once per MG*128 rows, ring of up to 16 stages;
+// One kernel, k_g2_conv: a CTA owns a super-tile of NG x MG m-tiles (128 rows each) x nt <= 128 columns, NG*MG*nt <= 128 columns of
+// fp32 accumulator image in shared memory (the whole accumulator of the super-tile), so each weight stage (chunk c, tap j) feeds MG
+// 128-row MMAs:
+//   streamed weights (C >= 64): NG = 1, MG = 128/nt -- weights cross L2->SM once per MG*128 rows, ring of up to 16 stages;
 //   resident weights (C <= 32): all taps loaded once, the M-groups pipeline through the activation ring and the tail of
 //   group g overlaps the MMAs of group g+1.
-// 512 threads: warp 0 activation producer, warp 1 MMA issuer, warp 2 weight producer, warp 3 TMEM allocator,
-// warps 4-15 epilogue (accumulator init with the bias before the MMAs; tail TMEM -> [+ residual] [+ MRF running sum] -> lrelu -> f16
+// 640 threads: warp 0 activation producer, warp 2 weight producer, warp 3 output halo, warps 16-19 MMA warpgroup (warp 1 idle),
+// warps 4-15 epilogue (accumulator init with the bias before the MMAs; tail accumulator image -> [+ residual] [+ MRF running sum] -> lrelu -> f16
 // -> 16-byte coalesced stores).
 #pragma once
 #include "tc_conv.cuh"
@@ -42,11 +43,11 @@ struct G2Params {
     const uint4* x; uint4* y; const uint4* res; const void* w; const float* bias; const float* bias_b;
     int x_cg, x_Tp, y_cg, y_Tp, res_cg, res_Tp, bias_b_stride;
     int T, K, dil, pad, nt, KC, nchunks, NG, MG, R, nas, nws, resident;
-    uint32_t a_stage_bytes, w_stage_bytes, tmem_cols, idesc;
+    uint32_t a_stage_bytes, w_stage_bytes, acc_cols;  // acc_cols: columns of the accumulator image
     int residual, accumulate, ups_u, ups_cout;
     float out_scale;
     int dbg_skip_wcommit;  // probes only: no weight-stage commits (valid only when every weight stage fits the ring)
-    int dbg_flags;         // probes only (timing studies, wrong results): 1 = no tap shift (aligned A operand), 2 = no tcgen05.fence after the stage waits,
+    int dbg_flags;         // probes only (timing studies, wrong results): 1 = no tap shift (aligned A operand), 2 = no wgmma fence after the stage waits,
                            // 4 = no TMA traffic after the first ring fill (stale operands re-used: isolates shared-memory contention), 8 = epilogue warps
                            // park in nanosleep polling instead of the hinted try_wait, 16 = no halo zeroing of the output
     long long* prof;  // probes only: per-CTA timestamps [grid][16] (globaltimer ns / clock64 sums); nullptr in the engine
@@ -62,35 +63,27 @@ __device__ __forceinline__ void unpack8(const uint4& u, float* f) {
 __device__ __forceinline__ float unlrelu10(float a) { return a >= 0.f ? a : a * 10.f; }
 }  // namespace tc
 
-// MMAs of one weight stage (chunk c, tap j): MG m-tiles x NK k-steps, both compile-time: the stage is straight-line code, every
-// UTCHMMA gets its own freshly computed uniform registers and nothing but independent UIADD3/UMOV sits between two MMAs.
-// (History, all measured with the in-kernel phase accounting of tests/cuda/g2_probe.cu, N = 128: per-thread issue path with an
-//  ELECT + R2UR waterfall per MMA 280-570 clk/MMA -> uniform registers 185 -> no runtime division per stage 162 -> this.  The uniform
-//  datapath issues one instruction at a time with ~10-cycle dependent latency: a guarded MMA (UISETP + BRA.U + address math) costs
-//  ~100 cycles of issuer time whatever its size, so loops over runtime MG with per-MMA predicates never reach the tensor rate.)
+// MMAs of one weight stage (chunk c, tap j): MG m-tiles x NK k-steps (NK compile-time), each m-tile one wg_mma over the
+// accumulator image.
 template <int NK, int MG>
-__device__ __forceinline__ void g2_issue_stage(uint32_t d0, uint32_t a_lo0, uint32_t b_lo0, uint32_t a_kstep, uint32_t b_kstep, uint64_t hi, uint32_t nt, uint32_t idesc) {
-#pragma unroll
-    for (int mt = 0; mt < MG; mt++) {
-#pragma unroll
-        for (int kk = 0; kk < NK; kk++)
-            tc::umma_el<1>(d0 + (uint32_t)mt * nt, hi | (a_lo0 + (uint32_t)(mt * 128) + kk * a_kstep), hi | (b_lo0 + kk * b_kstep), idesc, 1u);
-    }
+__device__ __forceinline__ void g2_issue_stage(uint32_t d0, uint32_t a_lo0, uint32_t b_lo0, uint32_t a_kstep, uint32_t b_kstep, uint64_t hi, uint32_t nt) {
+#pragma unroll 1
+    for (int mt = 0; mt < MG; mt++)
+        tc::wg_mma<1>(d0 + (uint32_t)mt * nt, hi | (a_lo0 + (uint32_t)(mt * 128)), hi | b_lo0, a_kstep, b_kstep, NK, (int)nt, 1u);
 }
 
 // State the MMA issuer carries through its loops (all warp-uniform)
 struct G2Issue {
     uint32_t bar_af, bar_ae, bar_wf, bar_we, bar_acc;      // first barrier of each group
     uint32_t a_lo_base, w_lo_base, a_stage16, w_stage16;   // descriptor low words of ring slot 0, slot strides (16-byte units)
-    uint32_t a_kstep, b_kstep, nt, idesc, tapstep, tm;
+    uint32_t a_kstep, b_kstep, nt, tapstep, tm;
     uint32_t nas, nws;
-    int NG, NCH, K, streamed, wcommit, nostale, nofence;
+    int NG, NCH, K, streamed, wcommit, nostale;
     uint64_t hi;
 };
 
 // The issuer's loop nest for one (NK, MG) instantiation.  Ring slots, parities, barrier addresses and descriptor words are carried
-// incrementally (adds and compares only; an earlier version recomputed slot = i % n, parity = (i / n) & 1 per stage: ~120 dependent
-// instructions of runtime integer division in front of every 2-8 MMAs, profiles/r02c_g2_ncu_full.md).
+// incrementally (adds and compares only: no runtime integer division in front of every stage's MMAs).
 template <int NK, int MG>
 __device__ __forceinline__ void g2_issuer(const G2Issue& q, long long* prof, int lane) {
     using namespace tc;
@@ -104,26 +97,24 @@ __device__ __forceinline__ void g2_issuer(const G2Issue& q, long long* prof, int
         for (int c = 0; c < q.NCH; c++, s++) {
             long long c0 = prof ? clock64() : 0;
             if (q.nostale || s < (int)q.nas) mbar_wait_u(q.bar_af + 8u * sa, aph);
-            fence_after();
             if (prof) { waitA += clock64() - c0; if (s == 0 && lane == 0) { prof[3] = gtime(); prof[10] = clock64(); } }
             uint32_t a_tap = a_cur;
             for (int j = 0; j < q.K; j++, wi++, a_tap += q.tapstep) {
                 if (q.streamed) {
                     c0 = prof ? clock64() : 0;
                     if (q.nostale || wi < (int)q.nws) mbar_wait_u(q.bar_wf + 8u * sw, wph);
-                    if (!q.nofence) fence_after();
                     if (prof) waitW += clock64() - c0;
                 }
-                g2_issue_stage<NK, MG>(dg, a_tap, w_cur, q.a_kstep, q.b_kstep, q.hi, q.nt, q.idesc);
-                if (q.wcommit) umma_commit_el(q.bar_we + 8u * sw);
+                g2_issue_stage<NK, MG>(dg, a_tap, w_cur, q.a_kstep, q.b_kstep, q.hi, q.nt);
+                if (q.wcommit) wg_commit(q.bar_we + 8u * sw);
                 w_cur += q.w_stage16;
                 if (q.streamed && ++sw == q.nws) { sw = 0; wph ^= 1u; w_cur = q.w_lo_base; }
             }
-            umma_commit_el(q.bar_ae + 8u * sa);
+            wg_commit(q.bar_ae + 8u * sa);
             a_cur += q.a_stage16;
             if (++sa == q.nas) { sa = 0; aph ^= 1u; a_cur = q.a_lo_base; }
         }
-        umma_commit_el(q.bar_acc + 8u * (uint32_t)g);
+        wg_commit(q.bar_acc + 8u * (uint32_t)g);
     }
     if (prof && lane == 0) { prof[4] = gtime(); prof[8] = waitA; prof[9] = waitW; prof[11] = clock64(); prof[12] = (long long)q.NG * q.NCH * q.K * MG * NK; }
 }
@@ -140,9 +131,10 @@ __device__ __forceinline__ void g2_issuer_mg(const G2Issue& q, int MG, long long
     }
 }
 
-__global__ void __launch_bounds__(512, 1) k_g2_conv(G2Params p) {
+__global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
     using namespace tc;
-    extern __shared__ __align__(1024) uint8_t smem[];
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + acc_img_bytes(p.acc_cols);  // behind the accumulator image
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;  // shfl: warp-uniform for the compiler
     const int NAS = p.nas, NWS = p.nws, NG = p.NG, MG = p.MG, NCH = p.nchunks, nt = p.nt, R = p.R;
     const int t0 = blockIdx.x * NG * MG * 128, ntile = blockIdx.y, n0 = ntile * nt, b = blockIdx.z;
@@ -156,7 +148,6 @@ __global__ void __launch_bounds__(512, 1) k_g2_conv(G2Params p) {
     auto BAR = [&](int i) { return bar0 + 8u * (uint32_t)i; };
     // barrier map: a_full[NAS], a_empty[NAS], w_full[NWS], w_empty[NWS], acc_full[NG], acc_init
     const int B_AFULL = 0, B_AEMPTY = NAS, B_WFULL = 2 * NAS, B_WEMPTY = 2 * NAS + NWS, B_ACC = 2 * NAS + 2 * NWS, B_INIT = B_ACC + NG;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + B_INIT + 1);
 
     if (threadIdx.x == 0) {
         for (int i = 0; i < NAS; i++) { mbar_init(BAR(B_AFULL + i), 1); mbar_init(BAR(B_AEMPTY + i), 1); }
@@ -165,14 +156,8 @@ __global__ void __launch_bounds__(512, 1) k_g2_conv(G2Params p) {
         mbar_init(BAR(B_INIT), 12 * 32);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 3) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(p.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    fence_before();
     __syncthreads();
-    fence_after();
-    const uint32_t tmem = *tmem_slot;
+    const uint32_t acc0 = 0;  // accumulator image base (acc_ptr)
     const int ncg = p.KC / 8;  // 16-byte channel groups per chunk
 
     if (warp == 0) {
@@ -225,27 +210,26 @@ __global__ void __launch_bounds__(512, 1) k_g2_conv(G2Params p) {
                 }
             }
         }
-    } else if (warp == 1) {
+    } else if (warp >= 16) {
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-        // ===== MMA issuer: all 32 lanes run the loops convergently (uniform registers), one elected lane issues (see elect_one)
+        // ===== MMA warpgroup (warps 16-19): all 128 threads run the loops together (wgmma is warpgroup-collective)
         // Descriptors are kept as (constant high word, 32-bit low word): start address >> 4 in bits [0,14), LBO >> 4 in [16,30) of the low
         // word; tap / m-tile / k-step offsets are plain 32-bit adds on the low word (shared memory addresses stay below 2^18), which the
         // compiler keeps in the uniform datapath.
         const uint32_t a_lo_c = (((uint32_t)R * 16u) >> 4) << 16, b_lo_c = (((uint32_t)nt * 16u) >> 4) << 16;
-        const uint32_t desc_hi = (128u >> 4) | (1u << 14);  // SBO = 128 B, descriptor version 1
+        const uint32_t desc_hi = 128u >> 4;  // SBO = 128 B
         const uint32_t a_kstep = 2u * (uint32_t)R, b_kstep = 2u * (uint32_t)nt;
-        const uint32_t tm = __shfl_sync(0xffffffffu, tmem, 0);
+        const uint32_t tm = acc0;
         const int nk = p.KC / 16;
-        if (p.resident) { mbar_wait_u(BAR(B_WFULL), 0); fence_after(); }
+        if (p.resident) mbar_wait_u(BAR(B_WFULL), 0);
         mbar_wait_u(BAR(B_INIT), 0);  // accumulators hold the bias: every MMA accumulates
-        fence_after();
         G2Issue q;
         q.bar_af = BAR(B_AFULL); q.bar_ae = BAR(B_AEMPTY); q.bar_wf = BAR(B_WFULL); q.bar_we = BAR(B_WEMPTY); q.bar_acc = BAR(B_ACC);
         q.a_lo_base = ((smem_u32(sA) & 0x3ffffu) >> 4) | a_lo_c; q.w_lo_base = ((smem_u32(sW) & 0x3ffffu) >> 4) | b_lo_c;
         q.a_stage16 = p.a_stage_bytes >> 4; q.w_stage16 = p.w_stage_bytes >> 4;
-        q.a_kstep = a_kstep; q.b_kstep = b_kstep; q.nt = (uint32_t)nt; q.idesc = p.idesc; q.tapstep = (p.dbg_flags & 1) ? 0u : (uint32_t)p.dil; q.tm = tm;
+        q.a_kstep = a_kstep; q.b_kstep = b_kstep; q.nt = (uint32_t)nt; q.tapstep = (p.dbg_flags & 1) ? 0u : (uint32_t)p.dil; q.tm = tm;
         q.nas = (uint32_t)NAS; q.nws = (uint32_t)NWS; q.NG = NG; q.NCH = NCH; q.K = p.K;
-        q.streamed = !p.resident; q.wcommit = q.streamed && !p.dbg_skip_wcommit; q.nostale = !(p.dbg_flags & 4); q.nofence = (p.dbg_flags & 2) ? 1 : 0;
+        q.streamed = !p.resident; q.wcommit = q.streamed && !p.dbg_skip_wcommit; q.nostale = !(p.dbg_flags & 4);
         q.hi = (uint64_t)desc_hi << 32;
         if (nk == 2) g2_issuer_mg<2>(q, MG, prof, lane);
         else g2_issuer_mg<1>(q, MG, prof, lane);  // g2_conv() admits KC = 16 or 32 only
@@ -263,16 +247,16 @@ __global__ void __launch_bounds__(512, 1) k_g2_conv(G2Params p) {
             if (blockIdx.x == gridDim.x - 1)
                 for (int i = lane; i < p.y_cg * G2_PADR; i += 32) yb[(size_t)(i / G2_PADR) * p.y_Tp + Tout + (i % G2_PADR)] = z4;
         }
-    } else if (warp >= 4) {
-        // ===== epilogue, 12 warps: TMEM lane quarter q = warp & 3; the 3 warps of a quarter share the (m-tile, 32-column batch) items
+    } else if (warp >= 4 && warp < 16) {
+        // ===== epilogue, 12 warps: row quarter q = warp & 3; the 3 warps of a quarter share the (m-tile, 32-column batch) items
         // round-robin.  Two phases:
-        //   init (before the MMAs, before the PDL wait: touches only static data and CTA-private TMEM): the accumulators are pre-loaded
-        //        with bias (+ per-batch bias) by tcgen05.st, so every MMA accumulates and the tail has no bias loads / adds;
-        //   tail: TMEM -> [+ residual] [+ MRF running sum] -> lrelu -> f16 -> coalesced 16-byte stores.
+        //   init (before the MMAs, before the PDL wait: touches only static data and the CTA-private accumulator image): the accumulators are pre-loaded
+        //        with bias (+ per-batch bias) by image stores, so every MMA accumulates and the tail has no bias loads / adds;
+        //   tail: the accumulator image -> [+ residual] [+ MRF running sum] -> lrelu -> f16 -> coalesced 16-byte stores.
         // The tail is instruction-bound (two-three warps per scheduler cannot hide ALU latency: round-2 ncu), so it is kept lean.
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
         const int e = warp - 4, q = warp & 3, part = e >> 2;
-        const uint32_t trow = tmem + ((uint32_t)(q * 32) << 16);
+        const uint32_t trow = acc0 + ((uint32_t)(q * 32) << 16);
         const int u = p.ups_u;
         const int ncb = nt >= 32 ? nt / 32 : 1, cw = nt >= 32 ? 32 : 16;  // column batches per m-tile, columns per batch
         {
@@ -292,11 +276,9 @@ __global__ void __launch_bounds__(512, 1) k_g2_conv(G2Params p) {
                     }
                 }
                 for (int m = 0; m < NG * MG; m++) {
-                    if (cw == 32) tmem_st32(trow + (uint32_t)(m * nt + col0), v); else tmem_st16(trow + (uint32_t)(m * nt + col0), v);
+                    if (cw == 32) acc_st<32>(trow + (uint32_t)(m * nt + col0), v); else acc_st<16>(trow + (uint32_t)(m * nt + col0), v);
                 }
             }
-            tmem_wait_st();
-            fence_before();
             mbar_arrive(BAR(B_INIT));
         }
         asm volatile("griddepcontrol.wait;" ::: "memory");
@@ -309,7 +291,6 @@ __global__ void __launch_bounds__(512, 1) k_g2_conv(G2Params p) {
                     if (!done) __nanosleep(2000);
                 }
             } else mbar_wait(BAR(B_ACC + g), 0);
-            fence_after();
             if (prof && e == 0 && lane == 0 && g == 0) prof[5] = gtime();
             if (prof && e == 0 && lane == 0 && g == NG - 1) prof[6] = gtime();
             for (int it = part; it < MG * ncb; it += 3) {
@@ -317,8 +298,8 @@ __global__ void __launch_bounds__(512, 1) k_g2_conv(G2Params p) {
                 const int t = t0 + (g * MG + mt) * 128 + q * 32 + lane;
                 const bool ok = t < p.T;
                 uint32_t v[32];
-                if (cw == 32) tmem_ld32(trow + (uint32_t)((g * MG + mt) * nt + col0), v); else tmem_ld16(trow + (uint32_t)((g * MG + mt) * nt + col0), v);
-                // residual / running-sum operands are fetched while the TMEM load is in flight
+                if (cw == 32) acc_ld<32>(trow + (uint32_t)((g * MG + mt) * nt + col0), v); else acc_ld<16>(trow + (uint32_t)((g * MG + mt) * nt + col0), v);
+                // residual / running-sum operands are fetched while the accumulator image load is in flight
                 uint4 r4[4], a4[4];
                 size_t yo[4];
 #pragma unroll
@@ -331,7 +312,6 @@ __global__ void __launch_bounds__(512, 1) k_g2_conv(G2Params p) {
                         if (p.accumulate && ok) a4[h] = p.y[yo[h]];
                     }
                 }
-                tmem_wait_ld();
                 if (!ok) continue;
 #pragma unroll
                 for (int h = 0; h < 4; h++) {
@@ -366,11 +346,7 @@ __global__ void __launch_bounds__(512, 1) k_g2_conv(G2Params p) {
         }
     }
     if (prof && warp == 4 && lane == 0) prof[7] = gtime();
-    fence_before();
     __syncthreads();
-    if (warp == 3) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(p.tmem_cols) : "memory");
-    }
 }
 
 // ---- halo zeroing as a separate launch (probes; the engine's producers clear the halos of their own outputs, see k_g2_conv warp 3): the zero
@@ -480,9 +456,9 @@ inline void g2_conv(const TcConvW& w, const float* bias, const H8& x, const H8& 
     p.nt = w.nt; p.KC = w.KC; p.nchunks = w.nchunks;
     const int ntiles = w.Cout / w.nt, halo = (w.K - 1) * e.dil;
     p.w_stage_bytes = (uint32_t)(w.KC * w.nt * 2);
-    p.idesc = tc::make_idesc(1, w.nt);
-    const int mtiles = cdiv(x.T, 128), mgmax = 512 / w.nt;
-    const size_t budget = 220 * 1024;
+    // the accumulator image of a CTA holds at most 128 columns of 128 rows (66 KB of shared memory)
+    const int mtiles = cdiv(x.T, 128), mgmax = std::max(1, 128 / w.nt);
+    const size_t img = tc::acc_img_bytes((uint32_t)(mgmax * w.nt)), budget = 220 * 1024 - img;
     const size_t w_all = (size_t)w.nchunks * w.K * p.w_stage_bytes;
     p.resident = w_all <= 48 * 1024 && ntiles == 1;
     // ---- super-tile (m-tiles per CTA): as few CTAs as fill the SMs once; streamed weights want >= 2 m-tiles per weight pass
@@ -519,13 +495,12 @@ inline void g2_conv(const TcConvW& w, const float* bias, const H8& x, const H8& 
     if (p.resident) p.nws = 1;
     else p.nws = (int)std::max<size_t>(2, std::min<size_t>(16, (budget - (size_t)nas * p.a_stage_bytes - 1024) / p.w_stage_bytes));
     if (!p.resident) p.nws = std::min(p.nws, NG * w.nchunks * w.K);
-    uint32_t cols = 32; while ((int)cols < NG * MG * w.nt) cols <<= 1;
-    p.tmem_cols = cols;
-    const size_t smem = (size_t)nas * p.a_stage_bytes + (p.resident ? w_all : (size_t)p.nws * p.w_stage_bytes) + (size_t)(2 * nas + 2 * p.nws + NG + 3) * 8 + 16;
-    BV2_CHECK(smem <= 227 * 1024 && cols <= 512, "g2_conv shared memory / TMEM");
+    p.acc_cols = (uint32_t)(NG * MG * w.nt);
+    const size_t smem = tc::acc_img_bytes(p.acc_cols) + (size_t)nas * p.a_stage_bytes + (p.resident ? w_all : (size_t)p.nws * p.w_stage_bytes) + (size_t)(2 * nas + 2 * p.nws + NG + 3) * 8 + 16;
+    BV2_CHECK(smem <= 227 * 1024, "g2_conv shared memory");
     dim3 grid(cdiv(mtiles, NG * MG), ntiles, x.B);
     if (e.dbg_skip_wcommit && !p.resident && p.nws >= NG * w.nchunks * w.K) p.dbg_skip_wcommit = 1;
-    launch_pdl(k_g2_conv, grid, dim3(512), smem, st, p);
+    launch_pdl(k_g2_conv, grid, dim3(640), smem, st, p);
 }
 
 }  // namespace bv2

@@ -51,8 +51,8 @@ def _ptr(t: Optional[torch.Tensor]):
 
 
 class Engine:
-    """One engine per CUDA device.  precision: 'fp32' (SIMT FMA everywhere), 'tf32' (tcgen05 implicit-GEMM convs with TF32
-    operands) or 'fp16' (tcgen05 with FP16 operands -- same 11-bit significand as TF32, twice the tensor rate, half the
+    """One engine per CUDA device.  precision: 'fp32' (SIMT FMA everywhere), 'tf32' (wgmma implicit-GEMM convs with TF32
+    operands) or 'fp16' (wgmma with FP16 operands -- same 11-bit significand as TF32, twice the tensor rate, half the
     operand traffic; fp32 accumulate and fp32 activations in HBM).  Everything that feeds ceil(durations) is FP32 FMA in all three."""
 
     def __init__(self, cfg: ModelConfig, state_dict: Optional[Dict[str, torch.Tensor]], device="cuda:0", precision: str = "fp16",
@@ -61,7 +61,7 @@ class Engine:
         self.cfg = cfg
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise Bv2Error("bert_vits2_b200 has no CPU path: a CUDA (sm_100) device is required")
+            raise Bv2Error("bert_vits2_b200 has no CPU path: a CUDA (sm_90) device is required")
         idx = self.device.index if self.device.index is not None else torch.cuda.current_device()
         self.device = torch.device("cuda", idx)
         self.precision = PRECISIONS[precision]
@@ -69,7 +69,7 @@ class Engine:
         cs = _cfg_struct(cfg, self.precision)
         rc = self.lib.bv2_create(C.byref(self._h), C.byref(cs), idx)
         if rc != 0:
-            raise Bv2Error(f"bv2_create failed ({rc}): needs an sm_100 CUDA device, there is no fallback")
+            raise Bv2Error(f"bv2_create failed ({rc}): needs an sm_90 CUDA device, there is no fallback")
         if packed_path is not None:  # pre-folded, pre-packed weight file written by save_packed(): load = one cudaMemcpy
             self._check(self.lib.bv2_load_packed(self._h, os.fsencode(packed_path)))
             return

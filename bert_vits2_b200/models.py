@@ -10,7 +10,7 @@ Mirrors (names, argument meaning, return values, error behaviour):
   * .infer(...): reference models.py:1026-1074, same signature, returns
         (o [B,1,L], attn [B,1,F,T], y_mask [B,1,F], (z, z_p, m_p, logs_p))
 
-Only tensor plumbing happens here.  All arithmetic runs in libbv2.so (CUDA, sm_100a); there is no PyTorch or
+Only tensor plumbing happens here.  All arithmetic runs in libbv2.so (CUDA, sm_90a); there is no PyTorch or
 CPU fallback — calling .infer() on a CPU module raises.
 """
 from __future__ import annotations

@@ -2,7 +2,7 @@
 models.py:1026-1074), so the path shards embarrassingly -- one process per GPU, full weight replica per rank, no
 data-path collective.  The single exchange step is the collection of the finished waveforms on one rank (SURVEY.md
 §8e); the reference has no equivalent (inference is single-device, webui.py:31, 397-399).  Two implementations:
-`PeerWaveSlab` (B200-native: the Generator's conv_post+tanh epilogue stores into the root GPU's memory over
+`PeerWaveSlab` (the Generator's conv_post+tanh epilogue stores into the root GPU's memory over
 NVLink/NVSwitch through a CUDA-IPC mapped slab, NCCL carries only a 4-byte completion flag) and `gather_waveforms`
 (backend-agnostic padded gather; gloo in the CPU tests).
 

@@ -1,4 +1,4 @@
-/* libbv2 -- C ABI of the Blackwell-native VITS2 inference engine (Bert-VITS2 v2.3 `SynthesizerTrn.infer`).
+/* libbv2 -- C ABI of the Hopper-native (sm_90a) VITS2 inference engine (Bert-VITS2 v2.3 `SynthesizerTrn.infer`).
  *
  * The reference has no FFI/plugin layer: its seam is the Python class `models.SynthesizerTrn`
  * (reference models.py:811-1074) constructed by `infer.get_net_g` (reference infer.py:84-104) and driven by
@@ -12,7 +12,7 @@
  * (a cudaStream_t passed as void*); the only host synchronisation is inside bv2_infer_begin (one read-back of
  * y_lengths, the same data-dependent length the reference syncs on at models.py:1058 / commons.py:120-121).
  * One engine per device; concurrent callers are serialised by an internal mutex (ctypes drops the GIL).
- * There is NO CPU fallback: creation fails if no sm_100 device is present.
+ * There is NO CPU fallback: creation fails if no sm_90 (H100) device is present.
  */
 #ifndef BV2_H_
 #define BV2_H_
@@ -51,8 +51,8 @@ typedef struct {
     int32_t sdp_filter, sdp_kernel, sdp_n_flows, sdp_dds_layers, sdp_num_bins;
     float sdp_tail_bound;
     int32_t dp_filter, dp_kernel, cond_layer_idx;
-    int32_t generator_precision; /* 0 = fp32 SIMT convs; 1 = TF32 tcgen05 implicit-GEMM convs (flow + Generator); 2 = FP16-operand
-                                    tcgen05 convs (same 11-bit significand as TF32, fp32 accumulate, fp32 activations in HBM) */
+    int32_t generator_precision; /* 0 = fp32 SIMT convs; 1 = TF32 wgmma implicit-GEMM convs (flow + Generator); 2 = FP16-operand
+                                    wgmma convs (same 11-bit significand as TF32, fp32 accumulate, fp32 activations in HBM) */
     int32_t n_flows;             /* couplings in `flow`: n_flow_layer for TransformerCouplingBlock (models.py:82-145), always 4 for
                                     ResidualCouplingBlock, whose n_layers argument receives n_flow_layer (models.py:403-445, 918-919) */
 } bv2_config;
@@ -71,7 +71,7 @@ int bv2_finalize(bv2_engine* e);
 
 /* Packed engine weight file (SURVEY.md section 8f.4; the reference's only checkpoint tool is compress_model.py:44-53, which drops enc_q and
  * casts to fp16).  bv2_save_packed dumps the finalized engine's weight arena: weight-norm and Flip already folded, SIMT and
- * tcgen05 operand images already packed for this configuration + precision.  bv2_load_packed replaces the
+ * tensor-core operand images already packed for this configuration + precision.  bv2_load_packed replaces the
  * bv2_set_weight... + bv2_finalize sequence on a fresh engine created with the SAME bv2_config: it rebuilds the (cheap) layout
  * bookkeeping and fills device memory with ONE cudaMemcpy of the file image.  Mismatching configurations are rejected. */
 int bv2_save_packed(bv2_engine* e, const char* path);

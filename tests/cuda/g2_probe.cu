@@ -1,7 +1,7 @@
 // Standalone hardware probe for the 16-bit-activation Generator conv kernel (bert_vits2_b200/csrc/tc_gen.cuh): k_g2_conv against a
 // CPU conv on the identical f16 operands (plain / residual / MRF-accumulate / polyphase-upsample tails, streamed and resident
 // weights, super-tile sizes), halo zeroing, and timings of the Generator's shapes at config 2 (F = 1023 frames).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -DBV2_TUNING -o tests/cuda/g2_probe tests/cuda/g2_probe.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -DBV2_TUNING -o tests/cuda/g2_probe tests/cuda/g2_probe.cu
 // Run:   tests/cuda/g2_probe [perf]
 #include <cstdio>
 #include <cstdlib>

@@ -26,7 +26,7 @@ def test_library_exports_every_header_symbol(lib):
     assert declared == set(_lib.SYMBOLS), declared ^ set(_lib.SYMBOLS)
     for name in declared:
         assert hasattr(lib, name), name
-    assert b"sm_100a" in lib.bv2_version()
+    assert b"sm_90a" in lib.bv2_version()
 
 
 def test_create_fails_loudly_without_gpu(lib):

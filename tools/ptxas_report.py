@@ -6,7 +6,7 @@ import sys
 
 src = sys.argv[1] if len(sys.argv) > 1 else "bert_vits2_b200/csrc/engine.cu"
 extra = sys.argv[2:]
-cmd = ["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v",
+cmd = ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v",
        "-o", "/tmp/ptxas_report.so", src] + extra
 out = subprocess.run(cmd, capture_output=True, text=True).stderr
 cur = None
