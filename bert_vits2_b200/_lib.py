@@ -14,6 +14,9 @@ TUNING_LIB_PATH = os.path.join(HERE, "libbv2_tuning.so")  # development build (-
 SOURCES = [os.path.join(HERE, "csrc", "engine.cu")]
 HEADERS = sorted(os.path.join(HERE, "csrc", f) for f in os.listdir(os.path.join(HERE, "csrc")) if f.endswith(".cuh")) + [
     os.path.join(ROOT, "include", "bv2.h")]
+# kernel test harness (tests/cuda/kernel_harness.cu): the product headers behind an extern "C" test interface, same flags
+HARNESS_SOURCE = os.path.join(ROOT, "tests", "cuda", "kernel_harness.cu")
+HARNESS_PATH = os.path.join(HERE, "libbv2_kernel_harness.so")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
 MAX_UPS, MAX_RK, MAX_DIL = 8, 4, 4
@@ -98,6 +101,26 @@ def build(force: bool = False, verbose: bool = False, tuning: bool = False) -> s
         if verbose:
             print(r.stderr)
         return out
+
+
+def harness_needs_build() -> bool:
+    if not os.path.isfile(HARNESS_PATH):
+        return True
+    t = os.path.getmtime(HARNESS_PATH)
+    return any(os.path.getmtime(p) > t for p in [HARNESS_SOURCE] + HEADERS if os.path.isfile(p))
+
+
+def build_harness(force: bool = False) -> str:
+    """Compile the kernel test harness next to libbv2.so with the product flags (no -DBV2_TUNING)."""
+    with _lock:
+        if not force and not harness_needs_build():
+            return HARNESS_PATH
+        tmp = HARNESS_PATH + ".tmp"
+        r = subprocess.run(["nvcc"] + NVCC_FLAGS + ["-o", tmp, HARNESS_SOURCE], capture_output=True, text=True)
+        if r.returncode != 0:
+            raise RuntimeError("nvcc failed (kernel harness):\n" + r.stdout + r.stderr)
+        os.replace(tmp, HARNESS_PATH)
+        return HARNESS_PATH
 
 
 def load():

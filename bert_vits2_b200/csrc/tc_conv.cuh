@@ -1146,14 +1146,30 @@ inline int* tc_init_device() {
     return h;
 }
 
+// Which kernel a tc_conv1d call runs and with what pipeline shape.  tc_conv_plan() is a pure host function of the shapes, the epilogue
+// flags and num_sms (no device access), so a test can state which variant a case reaches.
+enum TcKind { TC_ONE_TILE = 0, TC_PERSIST = 1, TC_PSTREAM = 2 };
+struct TcConvPlan {
+    int kind = TC_ONE_TILE;
+    int gen = 0, f16 = 0;   // template arguments: generic epilogue, FP16 operands
+    int res_smem = 0;       // LayerNorm tail with the residual tile staged in shared memory
+    int nas = 0, nws = 0;   // activation / weight ring stages (persist: weights resident, nws = 0)
+    size_t smem = 0;        // dynamic shared memory per CTA
+    dim3 grid, block;
+    int mtiles = 0, ntiles = 0, total = 0;  // persistent kernels: 128-row tiles per batch row, N tiles, tiles in all
+};
+
 // x: c4 input [B][x.C/4][T][4]; y: c4 output ([B][y.C/4][T*max(1,ups_u)][4]).  Channel windows via e.cin_off/e.cout_off.
 // With e.in_f16 / e.out_f16 the tensor is the 16-bit c8 form [B][C/8][T][8] (Act.p reinterpreted).
-inline void tc_conv1d(const TcConvW& w, const float* bias, const Act& x, const Act& y, const TcEpi& e, cudaStream_t st, int num_sms) {
+// Fills the kernel parameters p and returns the plan; throws on an unsupported combination.
+inline TcConvPlan tc_conv_plan(const TcConvW& w, const float* bias, const Act& x, const Act& y, const TcEpi& e, int num_sms, TcParams& p) {
     const int u = w.ups_u ? w.ups_u : 1;
     const int F16 = w.f16;
     BV2_CHECK(w.w && x.B == y.B && y.T == x.T * u, "tc_conv1d shapes");
     BV2_CHECK(e.cin_off % 4 == 0 && e.cout_off % 4 == 0 && e.cin_off + w.Cin <= x.C, "tc_conv1d channel window");
-    TcParams p{};
+    p = TcParams{};
+    TcConvPlan pl;
+    pl.f16 = F16;
     p.x = x.p; p.y = y.p; p.w = w.w; p.bias = bias; p.res = e.res; p.bias_b = e.bias_b; p.lens = e.lens;
     p.Cin_total = x.C; p.cin_off = e.cin_off; p.Cout_total = y.C; p.cout_off = e.cout_off;
     p.res_C_total = e.res_C_total ? e.res_C_total : y.C; p.res_c_off = e.res_c_off; p.bias_b_stride = e.bias_b_stride;
@@ -1176,6 +1192,7 @@ inline void tc_conv1d(const TcConvW& w, const float* bias, const Act& x, const A
     if (p.in_mask || p.out_mask) BV2_CHECK(e.lens != nullptr, "mask needs lens");
     BV2_CHECK(!(p.relu && (p.res_mode || p.accumulate)), "relu cannot be combined with residual/accumulate (accumulator-init fusion)");
     const bool generic = w.ups_u || e.bias_b || e.relu || e.out_f16 || e.ln_gamma || e.gate;
+    pl.gen = generic ? 1 : 0;
     const uint32_t esz = F16 ? 2u : 4u;
     p.w_stage_bytes = (uint32_t)(p.KC * nt) * esz;
     auto set_rows = [&](int MT) {
@@ -1197,9 +1214,9 @@ inline void tc_conv1d(const TcConvW& w, const float* bias, const Act& x, const A
         const int mtiles = cdiv(p.T, 128);
         const int total = mtiles * p.B;
         const int grid_p = std::min(total, per_sm * num_sms);
-        if (generic) launch_pdl(F16 ? k_tc_conv1d_persist<1, 1> : k_tc_conv1d_persist<1, 0>, dim3(grid_p), dim3(512), smem_p, st, p, mtiles, total);
-        else launch_pdl(F16 ? k_tc_conv1d_persist<0, 1> : k_tc_conv1d_persist<0, 0>, dim3(grid_p), dim3(512), smem_p, st, p, mtiles, total);
-        return;
+        pl.kind = TC_PERSIST; pl.nas = p.nas; pl.nws = 0; pl.smem = smem_p; pl.grid = dim3(grid_p); pl.block = dim3(512);
+        pl.mtiles = mtiles; pl.ntiles = 1; pl.total = total;
+        return pl;
     }
     // ---- wide layer with at least one tile per SM: persistent CTAs, continuously streamed weights, double-buffered accumulator image
     // (only when two activation and two weight stages fit next to the double-buffered accumulator image; otherwise one tile per CTA)
@@ -1221,9 +1238,9 @@ inline void tc_conv1d(const TcConvW& w, const float* bias, const Act& x, const A
         const int mtiles = cdiv(p.T, 128 * MT);
         const int total = mtiles * p.B * ntiles;
         const int grid_s = std::min(total, num_sms);
-        if (generic) launch_pdl(F16 ? k_tc_conv1d_pstream<1, 1> : k_tc_conv1d_pstream<1, 0>, dim3(grid_s), dim3(512), smem_s, st, p, mtiles, ntiles, total);
-        else launch_pdl(F16 ? k_tc_conv1d_pstream<0, 1> : k_tc_conv1d_pstream<0, 0>, dim3(grid_s), dim3(512), smem_s, st, p, mtiles, ntiles, total);
-        return;
+        pl.kind = TC_PSTREAM; pl.nas = p.nas; pl.nws = p.nws; pl.smem = smem_s; pl.grid = dim3(grid_s); pl.block = dim3(512);
+        pl.mtiles = mtiles; pl.ntiles = ntiles; pl.total = total;
+        return pl;
     }
     // ---- one tile per CTA.  Shared memory per CTA is capped (~48 KB) when there are more CTAs than SMs so that several
     // CTAs co-reside: one CTA's accumulator init / tail overlaps the other's MMA main loop
@@ -1249,9 +1266,26 @@ inline void tc_conv1d(const TcConvW& w, const float* bias, const Act& x, const A
     size_t smem = img + (size_t)p.nas * p.a_stage_bytes + (size_t)p.nws * p.w_stage_bytes + (size_t)(3 * p.nas + 2 * p.nws + 3) * 8 + 16;
     if (res_smem) { smem = (smem + 15) & ~(size_t)15; p.res_soff = (uint32_t)(smem - img); smem += res_bytes; }  // offset from the kernel's `smem` (behind the image)
     BV2_CHECK(smem <= 227 * 1024, "tc_conv1d shared memory");
-    dim3 grid(cdiv(p.T, 128), ntiles, p.B);
-    if (generic) launch_pdl(F16 ? k_tc_conv1d<1, 1> : k_tc_conv1d<1, 0>, grid, dim3(384), smem, st, p);
-    else launch_pdl(F16 ? k_tc_conv1d<0, 1> : k_tc_conv1d<0, 0>, grid, dim3(384), smem, st, p);
+    pl.kind = TC_ONE_TILE; pl.res_smem = res_smem ? 1 : 0; pl.nas = p.nas; pl.nws = p.nws; pl.smem = smem;
+    pl.grid = dim3(cdiv(p.T, 128), ntiles, p.B); pl.block = dim3(384);
+    pl.mtiles = cdiv(p.T, 128); pl.ntiles = ntiles; pl.total = pl.mtiles * ntiles * p.B;
+    return pl;
+}
+
+// Runs the kernel tc_conv_plan() picks.
+inline void tc_conv1d(const TcConvW& w, const float* bias, const Act& x, const Act& y, const TcEpi& e, cudaStream_t st, int num_sms) {
+    TcParams p;
+    const TcConvPlan pl = tc_conv_plan(w, bias, x, y, e, num_sms, p);
+    if (pl.kind == TC_PERSIST) {
+        if (pl.gen) launch_pdl(pl.f16 ? k_tc_conv1d_persist<1, 1> : k_tc_conv1d_persist<1, 0>, pl.grid, pl.block, pl.smem, st, p, pl.mtiles, pl.total);
+        else launch_pdl(pl.f16 ? k_tc_conv1d_persist<0, 1> : k_tc_conv1d_persist<0, 0>, pl.grid, pl.block, pl.smem, st, p, pl.mtiles, pl.total);
+    } else if (pl.kind == TC_PSTREAM) {
+        if (pl.gen) launch_pdl(pl.f16 ? k_tc_conv1d_pstream<1, 1> : k_tc_conv1d_pstream<1, 0>, pl.grid, pl.block, pl.smem, st, p, pl.mtiles, pl.ntiles, pl.total);
+        else launch_pdl(pl.f16 ? k_tc_conv1d_pstream<0, 1> : k_tc_conv1d_pstream<0, 0>, pl.grid, pl.block, pl.smem, st, p, pl.mtiles, pl.ntiles, pl.total);
+    } else {
+        if (pl.gen) launch_pdl(pl.f16 ? k_tc_conv1d<1, 1> : k_tc_conv1d<1, 0>, pl.grid, pl.block, pl.smem, st, p);
+        else launch_pdl(pl.f16 ? k_tc_conv1d<0, 1> : k_tc_conv1d<0, 0>, pl.grid, pl.block, pl.smem, st, p);
+    }
 }
 
 // TF32 batched GEMMs on c4 operands (attention of the tf32 engine).

@@ -440,12 +440,23 @@ struct G2Epi {
 inline int g2_nt(int cols) { int nt = std::min(cols, 128); while (cols % nt || nt % 16) nt -= 16; return nt; }
 inline int g2_kc(int Cin) { return Cin >= 128 ? 32 : 16; }
 
+// Launch shape of a g2_conv call.  g2_conv_plan() is a pure host function of the shapes and num_sms (no device access), so a test can
+// state which variant a case reaches.
+struct G2Plan {
+    int resident = 0;       // all weight taps loaded once (else streamed through a ring of nws stages)
+    int NG = 1, MG = 1;     // super-tile: NG groups of MG 128-row m-tiles per CTA
+    int nas = 0, nws = 0;   // activation / weight ring stages
+    size_t smem = 0;        // dynamic shared memory per CTA
+    dim3 grid;
+};
+
 // x: H8 input, y: H8 output (T_out = T * max(1, ups_u)).  w packed by tc_pack_weights / tc_pack_upsample with f16 = 1, nt = g2_nt, kc = g2_kc.
-inline void g2_conv(const TcConvW& w, const float* bias, const H8& x, const H8& y, const G2Epi& e, cudaStream_t st, int num_sms) {
+// Fills the kernel parameters p and returns the plan; throws on an unsupported combination.
+inline G2Plan g2_conv_plan(const TcConvW& w, const float* bias, const H8& x, const H8& y, const G2Epi& e, int num_sms, G2Params& p) {
     const int u = w.ups_u ? w.ups_u : 1;
     BV2_CHECK(w.w && w.f16 && bias && x.B == y.B && y.T == x.T * u && x.C == w.Cin && (w.ups_u ? y.C == w.ups_cout : y.C == w.Cout), "g2_conv shapes");
     BV2_CHECK(w.nt <= 128 && (w.KC == 16 || w.KC == 32) && x.C % 8 == 0 && y.C % 8 == 0, "g2_conv tiling (K chunk of 16 or 32 channels)");
-    G2Params p{};
+    p = G2Params{};
     p.x = x.p; p.y = y.p; p.w = w.w; p.bias = bias; p.bias_b = e.bias_b; p.bias_b_stride = e.bias_b_stride;
     p.x_cg = x.C / 8; p.x_Tp = x.Tp; p.y_cg = y.C / 8; p.y_Tp = y.Tp;
     if (e.res) { BV2_CHECK(!w.ups_u && e.res->C == y.C && e.res->T == y.T && e.res->B == y.B, "g2_conv residual"); p.res = e.res->p; p.res_cg = e.res->C / 8; p.res_Tp = e.res->Tp; p.residual = 1; }
@@ -498,9 +509,17 @@ inline void g2_conv(const TcConvW& w, const float* bias, const H8& x, const H8& 
     p.acc_cols = (uint32_t)(NG * MG * w.nt);
     const size_t smem = tc::acc_img_bytes(p.acc_cols) + (size_t)nas * p.a_stage_bytes + (p.resident ? w_all : (size_t)p.nws * p.w_stage_bytes) + (size_t)(2 * nas + 2 * p.nws + NG + 3) * 8 + 16;
     BV2_CHECK(smem <= 227 * 1024, "g2_conv shared memory");
-    dim3 grid(cdiv(mtiles, NG * MG), ntiles, x.B);
     if (e.dbg_skip_wcommit && !p.resident && p.nws >= NG * w.nchunks * w.K) p.dbg_skip_wcommit = 1;
-    launch_pdl(k_g2_conv, grid, dim3(640), smem, st, p);
+    G2Plan pl;
+    pl.resident = p.resident; pl.NG = NG; pl.MG = MG; pl.nas = nas; pl.nws = p.nws; pl.smem = smem;
+    pl.grid = dim3(cdiv(mtiles, NG * MG), ntiles, x.B);
+    return pl;
+}
+
+inline void g2_conv(const TcConvW& w, const float* bias, const H8& x, const H8& y, const G2Epi& e, cudaStream_t st, int num_sms) {
+    G2Params p;
+    const G2Plan pl = g2_conv_plan(w, bias, x, y, e, num_sms, p);
+    launch_pdl(k_g2_conv, pl.grid, dim3(640), pl.smem, st, p);
 }
 
 }  // namespace bv2
