@@ -17,6 +17,9 @@ HEADERS = sorted(os.path.join(HERE, "csrc", f) for f in os.listdir(os.path.join(
 # kernel test harness (tests/cuda/kernel_harness.cu): the product headers behind an extern "C" test interface, same flags
 HARNESS_SOURCE = os.path.join(ROOT, "tests", "cuda", "kernel_harness.cu")
 HARNESS_PATH = os.path.join(HERE, "libbv2_kernel_harness.so")
+# streaming harness (tests/cuda/stream_harness.cu): the Generator's window launches and wavefront planner, on top of the kernel harness
+STREAM_HARNESS_SOURCE = os.path.join(ROOT, "tests", "cuda", "stream_harness.cu")
+STREAM_HARNESS_PATH = os.path.join(HERE, "libbv2_stream_harness.so")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
 MAX_UPS, MAX_RK, MAX_DIL = 8, 4, 4
@@ -48,6 +51,8 @@ SYMBOLS = {
                                   C.c_float, C.c_float, F32P, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
     "bv2_infer_finish": (C.c_int, [P, F32P, C.c_int64, C.c_float, C.c_int32, F32P, F32P, F32P, F32P, F32P, F32P, F32P, C.c_void_p]),
     "bv2_infer_finish_pcm16": (C.c_int, [P, F32P, C.c_int64, C.c_float, C.c_int32, C.c_void_p, F32P, F32P, F32P, F32P, F32P, F32P, C.c_void_p]),
+    "bv2_infer_finish_stream": (C.c_int, [P, F32P, C.c_int64, C.c_float, C.c_int32, F32P, F32P, F32P, F32P, F32P, F32P, F32P, C.c_void_p]),
+    "bv2_stream_advance": (C.c_int, [P, C.c_int32, C.c_void_p, C.POINTER(C.c_int64)]),
     "bv2_wave_to_pcm16": (C.c_int, [P, C.c_int, C.c_int64, F32P, I64P, C.c_void_p, C.c_void_p]),
     "bv2_attn_path": (C.c_int, [P, F32P, C.c_void_p]),
     "bv2_reserve": (C.c_int, [P, C.c_int, C.c_int, C.c_int]),
@@ -103,24 +108,27 @@ def build(force: bool = False, verbose: bool = False, tuning: bool = False) -> s
         return out
 
 
-def harness_needs_build() -> bool:
-    if not os.path.isfile(HARNESS_PATH):
+def harness_needs_build(stream: bool = False) -> bool:
+    path = STREAM_HARNESS_PATH if stream else HARNESS_PATH
+    if not os.path.isfile(path):
         return True
-    t = os.path.getmtime(HARNESS_PATH)
-    return any(os.path.getmtime(p) > t for p in [HARNESS_SOURCE] + HEADERS if os.path.isfile(p))
+    t = os.path.getmtime(path)
+    deps = [HARNESS_SOURCE] + ([STREAM_HARNESS_SOURCE] if stream else []) + HEADERS
+    return any(os.path.getmtime(p) > t for p in deps if os.path.isfile(p))
 
 
-def build_harness(force: bool = False) -> str:
-    """Compile the kernel test harness next to libbv2.so with the product flags (no -DBV2_TUNING)."""
+def build_harness(force: bool = False, stream: bool = False) -> str:
+    """Compile the kernel test harness (stream=True: the streaming harness) next to libbv2.so with the product flags (no -DBV2_TUNING)."""
+    src, path = (STREAM_HARNESS_SOURCE, STREAM_HARNESS_PATH) if stream else (HARNESS_SOURCE, HARNESS_PATH)
     with _lock:
-        if not force and not harness_needs_build():
-            return HARNESS_PATH
-        tmp = HARNESS_PATH + ".tmp"
-        r = subprocess.run(["nvcc"] + NVCC_FLAGS + ["-o", tmp, HARNESS_SOURCE], capture_output=True, text=True)
+        if not force and not harness_needs_build(stream):
+            return path
+        tmp = path + ".tmp"
+        r = subprocess.run(["nvcc"] + NVCC_FLAGS + ["-o", tmp, src], capture_output=True, text=True)
         if r.returncode != 0:
-            raise RuntimeError("nvcc failed (kernel harness):\n" + r.stdout + r.stderr)
-        os.replace(tmp, HARNESS_PATH)
-        return HARNESS_PATH
+            raise RuntimeError(f"nvcc failed ({os.path.basename(src)}):\n" + r.stdout + r.stderr)
+        os.replace(tmp, path)
+        return path
 
 
 def load():

@@ -17,6 +17,7 @@
 #include "kernels_simt.cuh"
 #include "tc_conv.cuh"
 #include "tc_gen.cuh"
+#include "gen_stream.cuh"
 #include "tc_attn.cuh"
 #include "kernels_tok.cuh"
 
@@ -112,6 +113,22 @@ struct bv2_engine {
         float* stats = nullptr; int* cum = nullptr; long long* ylen = nullptr; int* ylen32 = nullptr; int* lens = nullptr;
         float* gproj = nullptr; float* w_ceil = nullptr;
     } st;
+    // Open Generator stream (bv2_infer_finish_stream .. the bv2_stream_advance that reaches Fg).  Every tensor of the Generator stays
+    // alive in the workspace for the stream's lifetime, because later windows read the rows behind each layer's done pointer: the
+    // input z plus conv_pre's output plus, per upsampling stage, the stage sum S, the upsampled xu and one tensor per resblock conv
+    // except the last of each chain (2 + 3 * (3 + 2) = 17 tensors per stage at the default configuration), against the one-shot
+    // Generator's per-stage release.  Per frame per utterance at the default configuration that is, besides z itself,
+    //   FP16 Generator (16-bit H8 tensors):  2 * (192 + 512 + 17 * (256*8 + 128*64 + 64*128 + 32*256 + 16*512)) = 1,185,152 bytes
+    //                                        plus the zero halo rows;
+    //   fp32 / TF32 Generator (fp32 c4):     4 * (512 + 17 * (256*8 + 128*64 + 64*128 + 32*256 + 16*512))       = 2,369,536 bytes.
+    // The stream also reads the per-batch conditioning and the lengths in the persist arena.  Any call that resets the workspace, and a
+    // bv2_reserve that regrows either arena, closes the stream.
+    struct {
+        bool open = false; int B = 0, Fg = 0, frontier = 0;
+        GenGraph g; std::vector<H8> t; std::vector<Act> a;  // tensors of the FP16 Generator (t) / of the fp32 c4 Generator (a)
+        float* o = nullptr; const float* gdec = nullptr; int g_stride = 0; const int* lens = nullptr;
+    } gs;
+    void ws_reset() { gs.open = false; ws.reset(); }
     long long* h_ylen = nullptr;  // pinned
     int* h_err = nullptr;         // pinned + mapped: device-side error flag (barrier timeouts), see tc_conv.cuh
     // side streams: the MRF's resblocks (k = 3, 7, 11) of one Generator stage are independent chains of 6 convs
@@ -299,7 +316,7 @@ struct bv2_engine {
             e.in_slope = extra.in_slope; e.in_mask = extra.in_mask; e.relu = extra.act == 1; e.res_mode = extra.res_mode; e.res = extra.res;
             e.res_C_total = extra.res_C_total; e.res_c_off = extra.res_c_off; e.accumulate = extra.accumulate; e.out_scale = extra.out_scale;
             e.out_mask = extra.out_mask; e.lens = extra.lens; e.bias_b = extra.bias_b; e.bias_b_stride = extra.bias_b_stride;
-            e.cin_off = cin_off; e.cout_off = cout_off; e.dil = extra.dil ? extra.dil : 1;
+            e.cin_off = cin_off; e.cout_off = cout_off; e.dil = extra.dil ? extra.dil : 1; e.t_begin = extra.t_begin; e.t_end = extra.t_end;
             e.out_tf32 = tc_out_tf32; e.skip_xform = tc_skip_xform; e.in_f16 = tc_in_f16; e.out_f16 = tc_out_f16;
             BV2_CHECK(x.T == y.T && x.B == y.B, "conv T/B mismatch");
             if (tc_ln) { e.ln_gamma = tc_ln->g; e.ln_beta = tc_ln->b; }
@@ -364,6 +381,15 @@ struct bv2_engine {
     void run_flow(Act z, const int* lens, const float* gproj, cudaStream_t s);
     void run_generator(Act z, const int* lens_or_null, const float* gdec, int g_stride, float* o, cudaStream_t s);
     void run_generator_g2(Act z, const int* lens_or_null, const float* gdec, int g_stride, float* o, cudaStream_t s);
+    H8 g2_h8(int B, int C, int T);
+    H8 g2_input(Act z, const int* lens_or_null, cudaStream_t s);
+    int gen_channels(const GenGraph& g, int tensor) const;
+    size_t gen_stream_bytes(int B, int Fg) const;
+    void gen_stream_open(Act z, const int* lens_or_null, const float* gdec, int g_stride, float* o, cudaStream_t s);
+    void gen_windows(const GenGraph& g, const std::vector<GenWin>& w, std::vector<Act>& t, bool stream, const int* lens_or_null, const float* gdec,
+                     int g_stride, float* o, cudaStream_t s);
+    void g2_windows(const GenGraph& g, const std::vector<GenWin>& w, std::vector<H8>& t, bool stream, const float* gdec, int g_stride,
+                    float* o, cudaStream_t s);
     int* lens_to_device(const int64_t* x_lengths_dev, int B, Arena& ar, cudaStream_t s);
     // ids inside their tables, 1 <= lengths <= T (the reference raises IndexError / a shape error): device-side check into *err_dev
     void launch_validate(int B, int T, const int64_t* x, const int64_t* tone, const int64_t* lang, const int64_t* sid, const int64_t* lens,
@@ -952,131 +978,246 @@ void bv2_engine::run_flow(Act z, const int* lens, const float* gproj, cudaStream
     ws.release(mark);
 }
 
-// Generator.forward (reference models.py:538-557) + ResBlock1.forward (modules.py:296-309)
+// Generator.forward (reference models.py:538-557) + ResBlock1.forward (modules.py:296-309).  The one-shot run is the one-chunk plan of a
+// stream (gen_stream.cuh): every window covers its whole layer.
 void bv2_engine::run_generator(Act z, const int* lens, const float* gdec, int g_stride, float* o, cudaStream_t s) {
     if (use_g2) { run_generator_g2(z, lens, gdec, g_stride, o, s); return; }
-    const int B = z.B, F = z.T;
-    int ch = cfg.upsample_initial_channel, L = F;
-    Act x = ws.act(B, ch, L);
-    ConvArgs a; a.bias_b = gdec; a.bias_b_stride = g_stride;
-    if (lens) { a.in_mask = 1; a.lens = lens; }
+    const GenGraph g = gen_graph(cfg, z.T);
+    std::vector<Act> t(g.tensor_len.size());
+    t[0] = z;
+    gen_windows(g, gen_stream_plan(g, z.T, 0, z.T), t, false, lens, gdec, g_stride, o, s);
+}
+
+// fp32 c4 Generator (SIMT, or TF32 wgmma with generator_precision 1) over the windows of w, on the tensors t (one per GenGraph tensor;
+// t[0] is the input z).  stream = false: a one-shot run over whole layers; the stage temporaries are bump-allocated per stage and
+// released after the join.  stream = true: a chunk of a stream, on tensors that live as long as the stream.  Zero padding is the
+// kernels' bounds check against each tensor's full length, so a window reads final rows or padding only (gen_stream.cuh).
+void bv2_engine::gen_windows(const GenGraph& g, const std::vector<GenWin>& w, std::vector<Act>& t, bool stream, const int* lens, const float* gdec,
+                             int g_stride, float* o, cudaStream_t s) {
+    const int B = t[0].B;
     const bool tc = cfg.generator_precision != 0;
-    conv(conv_pre, z, x, s, a, 0, 0, tc);
+    int li = 0;
+    // runs layer li over its window (nothing for an empty one) with the epilogue a
+    auto conv_layer = [&](const ConvW& cw, ConvArgs a, cudaStream_t sj) {
+        const GenLayer& l = g.layers[li];
+        const GenWin& wi = w[li++];
+        if (wi.t_end <= wi.t_begin) return;
+        a.t_begin = wi.t_begin; a.t_end = wi.t_end;
+        if (l.res >= 0) { a.res_mode = 1; a.res = t[l.res].p; a.res_C_total = t[l.res].C; }
+        conv(cw, t[l.in], t[l.out], sj, a, 0, 0, tc);
+    };
+    if (!stream) t[g.layers[0].out] = ws.act(B, cfg.upsample_initial_channel, g.layers[0].L_out);
+    {
+        ConvArgs a; a.bias_b = gdec; a.bias_b_stride = g_stride;
+        if (lens) { a.in_mask = 1; a.lens = lens; }
+        conv_layer(conv_pre, a, s);
+    }
     const int nk = cfg.n_resblock_kernels, nd = cfg.n_dilations;
     BV2_CHECK(nk <= 4, "at most 4 resblock kernels");
     ensure_side_streams();
     for (int i = 0; i < cfg.n_ups; i++) {
         const UpW& u = ups[i];
-        const int Lo = L * u.u;
-        Act S = ws.act(B, u.Cout, Lo);
-        const size_t mark_after_S = ws.used();  // stage temporaries are released after the join; S (next stage's input) stays
-        Act xu = ws.act(B, u.Cout, Lo);
-        ConvTArgs t; t.x = x.p; t.Cin = u.Cin; t.Tin = L; t.w = u.w; t.bias = u.b; t.y = xu.p; t.Cout = u.Cout; t.Tout = Lo;
-        t.K = u.K; t.u = u.u; t.p = (u.K - u.u) / 2; t.B = B; t.in_slope = 0.1f;
-        if (tc) {
-            TcEpi eu; eu.in_slope = 0.1f;
-            tc_conv1d(u.tc, u.b, x, xu, eu, s, num_sms); launches++;
-        } else {
-            dim3 grid(cdiv(Lo, 128), cdiv(u.Cout, 64), B);
-            k_convT_c4<<<grid, 256, 0, s>>>(t);
-            BV2_CUDA(cudaGetLastError()); launches++;
+        const GenLayer& lu = g.layers[li];
+        BV2_CHECK(lu.kind == GenLayer::UPS && lu.stage == i, "Generator plan order");
+        auto layer_of = [&](int j, int d, int c2) -> const GenLayer& { return g.layers[li + 1 + 2 * (j * nd + d) + c2]; };
+        size_t mark_after_S = 0;
+        if (!stream) {
+            const int Lo = lu.L_out;
+            t[layer_of(0, nd - 1, 1).out] = ws.act(B, u.Cout, Lo);  // S: the next stage's input stays
+            mark_after_S = ws.used();
+            t[lu.out] = ws.act(B, u.Cout, Lo);
+            for (int j = 0; j < nk; j++) {
+                const Act xt = ws.act(B, u.Cout, Lo), ra = ws.act(B, u.Cout, Lo), rb = ws.act(B, u.Cout, Lo);
+                for (int d = 0; d < nd; d++) {
+                    t[layer_of(j, d, 0).out] = xt;
+                    if (d < nd - 1) t[layer_of(j, d, 1).out] = d % 2 ? rb : ra;
+                }
+            }
+        }
+        {
+            const Act& x = t[lu.in];
+            const Act& xu = t[lu.out];
+            const GenWin& wi = w[li++];
+            if (wi.t_end > wi.t_begin) {
+                if (tc) {
+                    TcEpi eu; eu.in_slope = 0.1f; eu.t_begin = wi.t_begin; eu.t_end = wi.t_end;
+                    tc_conv1d(u.tc, u.b, x, xu, eu, s, num_sms); launches++;
+                } else {
+                    ConvTArgs ct; ct.x = x.p; ct.Cin = u.Cin; ct.Tin = x.T; ct.w = u.w; ct.bias = u.b; ct.y = xu.p; ct.Cout = u.Cout; ct.Tout = xu.T;
+                    ct.K = u.K; ct.u = u.u; ct.p = (u.K - u.u) / 2; ct.B = B; ct.in_slope = 0.1f; ct.n_begin = wi.t_begin; ct.n_end = wi.t_end;
+                    dim3 grid(cdiv(wi.t_end - wi.t_begin, 128), cdiv(u.Cout, 64), B);
+                    k_convT_c4<<<grid, 256, 0, s>>>(ct);
+                    BV2_CUDA(cudaGetLastError()); launches++;
+                }
+            }
         }
         // fork: resblock j runs on its own stream; only the last conv of each chain (the MRF running sum) is ordered
         BV2_CUDA(cudaEventRecord(ev_fork, s));
         for (int j = 0; j < nk; j++) {
             cudaStream_t sj = j == 0 ? s : side[j];
             if (j) BV2_CUDA(cudaStreamWaitEvent(sj, ev_fork, 0));
-            Act xt = ws.act(B, u.Cout, Lo), ra = ws.act(B, u.Cout, Lo), rb = ws.act(B, u.Cout, Lo);
             const ResBlockW& R = resblocks[i * nk + j];
-            Act cur = xu;
             for (int d = 0; d < nd; d++) {
                 const bool last = d == nd - 1;
-                Act nxt = last ? S : (cur.p == ra.p ? rb : ra);
-                if (tc) {
-                    TcEpi e1; e1.in_slope = 0.1f; e1.dil = R.dil[d];
-                    tc_conv1d(R.c1[d].tc, R.c1[d].b, cur, xt, e1, sj, num_sms); launches++;
-                    if (last && j > 0) BV2_CUDA(cudaStreamWaitEvent(sj, ev_rb[j - 1], 0));  // S += ... after resblock j-1 wrote S
-                    TcEpi e2; e2.in_slope = 0.1f; e2.res = cur.p; e2.res_mode = 1;
-                    if (last) { e2.accumulate = j > 0; e2.out_scale = (j == nk - 1) ? 1.f / nk : 1.f; }
-                    tc_conv1d(R.c2[d].tc, R.c2[d].b, xt, nxt, e2, sj, num_sms); launches++;
-                } else {
-                    ConvArgs c1; c1.in_slope = 0.1f; c1.dil = R.dil[d];
-                    conv(R.c1[d], cur, xt, sj, c1);
-                    if (last && j > 0) BV2_CUDA(cudaStreamWaitEvent(sj, ev_rb[j - 1], 0));
-                    ConvArgs c2; c2.in_slope = 0.1f; c2.res_mode = 1; c2.res = cur.p; c2.res_C_total = u.Cout;
-                    if (last) { c2.accumulate = j > 0; c2.out_scale = (j == nk - 1) ? 1.f / nk : 1.f; }
-                    conv(R.c2[d], xt, nxt, sj, c2);
-                }
-                cur = nxt;
+                ConvArgs c1; c1.in_slope = 0.1f; c1.dil = R.dil[d];
+                conv_layer(R.c1[d], c1, sj);
+                if (last && j > 0) BV2_CUDA(cudaStreamWaitEvent(sj, ev_rb[j - 1], 0));  // S += ... after resblock j-1 wrote S
+                ConvArgs c2; c2.in_slope = 0.1f;  // residual: the chain's input (GenLayer::res)
+                if (last) { c2.accumulate = j > 0; c2.out_scale = (j == nk - 1) ? 1.f / nk : 1.f; }
+                conv_layer(R.c2[d], c2, sj);
             }
             BV2_CUDA(cudaEventRecord(ev_rb[j], sj));
         }
         // join: the caller's stream continues after the last resblock (which itself waited for all earlier ones)
         if (nk > 1) BV2_CUDA(cudaStreamWaitEvent(s, ev_rb[nk - 1], 0));
-        if (i == 0) debug("gen_stage0", S);
-        x = S; L = Lo; ch = u.Cout;
-        ws.release(mark_after_S);
+        if (!stream) {
+            if (i == 0) debug("gen_stage0", t[layer_of(0, nd - 1, 1).out]);
+            ws.release(mark_after_S);
+        }
     }
-    dim3 grid(cdiv(L, 256), B);
-    k_conv_post_tanh<16, 7><<<grid, 256, 0, s>>>(x.p, conv_post_w, o, L, 0.01f);
-    BV2_CUDA(cudaGetLastError()); launches++;
+    const GenLayer& lp = g.layers[li];
+    BV2_CHECK(lp.kind == GenLayer::CONV_POST && li + 1 == (int)g.layers.size(), "Generator plan order");
+    const GenWin& wp = w[li];
+    if (wp.t_end > wp.t_begin) {
+        dim3 grid(cdiv(wp.t_end - wp.t_begin, 256), B);
+        k_conv_post_tanh<16, 7><<<grid, 256, 0, s>>>(t[lp.in].p, conv_post_w, o, lp.L_out, 0.01f, wp.t_begin, wp.t_end);
+        BV2_CUDA(cudaGetLastError()); launches++;
+    }
 }
 
 // Generator on 16-bit activation tensors (tc_gen.cuh): every tensor between conv_pre and conv_post is an H8 operand image
-// (f16(lrelu_0.1(x)), zero halos); 96 launches of ONE kernel (k_g2_conv) + conv_post.
+// (f16(lrelu_0.1(x)), zero halos); 96 launches of ONE kernel (k_g2_conv) + conv_post.  The one-shot run is the one-chunk plan of a
+// stream (gen_stream.cuh): every window covers its whole layer.
 void bv2_engine::run_generator_g2(Act z, const int* lens, const float* gdec, int g_stride, float* o, cudaStream_t s) {
-    const int B = z.B, F = z.T, I = z.C;
-    auto h8 = [&](int C, int T) {
-        H8 t; t.B = B; t.C = C; t.T = T; t.Tp = G2_PADL + T + G2_PADR;
-        t.p = reinterpret_cast<uint4*>(ws.alloc(H8::bytes(B, C, T) / 4)) + G2_PADL;
-        return t;
-    };
-    int ch = cfg.upsample_initial_channel, L = F;
-    H8 zh = h8(I, F), x = h8(ch, L);  // zero halos: every producer clears the halo rows of its own output (k_c4_to_h8, k_g2_conv)
-    k_c4_to_h8<<<dim3(cdiv(F, 128), I / 8, B), 128, 0, s>>>(reinterpret_cast<const float4*>(z.p), zh.p, I, F, zh.Tp, lens);
+    const GenGraph g = gen_graph(cfg, z.T);
+    std::vector<H8> t(g.tensor_len.size());
+    t[0] = g2_input(z, lens, s);
+    g2_windows(g, gen_stream_plan(g, z.T, 0, z.T), t, false, gdec, g_stride, o, s);
+}
+
+H8 bv2_engine::g2_h8(int B, int C, int T) {
+    H8 t; t.B = B; t.C = C; t.T = T; t.Tp = G2_PADL + T + G2_PADR;
+    t.p = reinterpret_cast<uint4*>(ws.alloc(H8::bytes(B, C, T) / 4)) + G2_PADL;
+    return t;
+}
+
+// z * y_mask as the raw f16 H8 tensor conv_pre reads (zero halos: every producer clears the halo rows of its own output)
+H8 bv2_engine::g2_input(Act z, const int* lens, cudaStream_t s) {
+    H8 zh = g2_h8(z.B, z.C, z.T);
+    k_c4_to_h8<<<dim3(cdiv(z.T, 128), z.C / 8, z.B), 128, 0, s>>>(reinterpret_cast<const float4*>(z.p), zh.p, z.C, z.T, zh.Tp, lens);
     BV2_CUDA(cudaGetLastError()); launches++;
+    return zh;
+}
+
+int bv2_engine::gen_channels(const GenGraph& g, int tensor) const {
+    if (tensor == 0) return cfg.inter_channels;
+    for (const GenLayer& l : g.layers)
+        if (l.out == tensor) return l.kind == GenLayer::CONV_PRE ? cfg.upsample_initial_channel : l.kind == GenLayer::CONV_POST ? 1 : ups[l.stage].Cout;
+    throw Error(BV2_ERR_INTERNAL, "gen_channels: unknown tensor");
+}
+
+// Workspace bytes of a stream's tensors (all but the waveform, which the caller owns, and, for the fp32 Generator, the input z,
+// which the caller allocated)
+size_t bv2_engine::gen_stream_bytes(int B, int Fg) const {
+    const GenGraph g = gen_graph(cfg, Fg);
+    size_t n = 0;
+    for (size_t i = use_g2 ? 0 : 1; i + 1 < g.tensor_len.size(); i++) {
+        const int C = gen_channels(g, (int)i), L = g.tensor_len[i];
+        n += ((use_g2 ? H8::bytes(B, C, L) : (size_t)B * C * L * sizeof(float)) + 255) & ~(size_t)255;
+    }
+    return n;
+}
+
+void bv2_engine::gen_stream_open(Act z, const int* lens, const float* gdec, int g_stride, float* o, cudaStream_t s) {
+    gs.g = gen_graph(cfg, z.T);
+    const size_t n = gs.g.tensor_len.size();
+    gs.t.clear(); gs.a.clear();
+    if (use_g2) {
+        gs.t.assign(n, H8());
+        gs.t[0] = g2_input(z, lens, s);
+        for (size_t i = 1; i + 1 < n; i++) gs.t[i] = g2_h8(z.B, gen_channels(gs.g, (int)i), gs.g.tensor_len[i]);
+    } else {
+        gs.a.assign(n, Act());
+        gs.a[0] = z;
+        for (size_t i = 1; i + 1 < n; i++) gs.a[i] = ws.act(z.B, gen_channels(gs.g, (int)i), gs.g.tensor_len[i]);
+    }
+    gs.B = z.B; gs.Fg = z.T; gs.frontier = 0; gs.o = o; gs.gdec = gdec; gs.g_stride = g_stride; gs.lens = lens;
+    gs.open = true;
+}
+
+// Runs every Generator layer over its window of w (GenGraph launch order; empty windows launch nothing) on the H8 tensors t, one per
+// GenGraph tensor.  stream = false: a one-shot run over whole layers; t holds only the input, and the stage temporaries are
+// bump-allocated per stage and released after the join (the convs of one resblock chain share one temporary and two ping-pong
+// buffers).  stream = true: a chunk of a stream, on tensors that live as long as the stream.
+void bv2_engine::g2_windows(const GenGraph& g, const std::vector<GenWin>& w, std::vector<H8>& t, bool stream, const float* gdec, int g_stride,
+                            float* o, cudaStream_t s) {
+    const int B = t[0].B;
+    int li = 0;
+    auto conv = [&](const TcConvW& cw, const float* bias, G2Epi e, cudaStream_t sj) {
+        const GenLayer& l = g.layers[li];
+        const GenWin& wi = w[li++];
+        if (wi.t_end <= wi.t_begin) return;
+        e.t_begin = wi.t_begin; e.t_end = wi.t_end;
+        if (l.res >= 0) e.res = &t[l.res];
+        g2_conv(cw, bias, t[l.in], t[l.out], e, sj, num_sms); launches++;
+    };
+    if (!stream) t[g.layers[0].out] = g2_h8(B, cfg.upsample_initial_channel, g.layers[0].L_out);
     {
         G2Epi e; e.bias_b = gdec; e.bias_b_stride = g_stride;
-        g2_conv(conv_pre.tc, conv_pre.b, zh, x, e, s, num_sms); launches++;
+        conv(conv_pre.tc, conv_pre.b, e, s);
     }
     const int nk = cfg.n_resblock_kernels, nd = cfg.n_dilations;
     BV2_CHECK(nk <= 4, "at most 4 resblock kernels");
     ensure_side_streams();
     for (int i = 0; i < cfg.n_ups; i++) {
         const UpW& u = ups[i];
-        const int Lo = L * u.u;
-        H8 S = h8(u.Cout, Lo);
-        const size_t mark_after_S = ws.used();
-        H8 xu = h8(u.Cout, Lo);
-        H8 xt[4], ra[4], rb[4];
-        for (int j = 0; j < nk; j++) { xt[j] = h8(u.Cout, Lo); ra[j] = h8(u.Cout, Lo); rb[j] = h8(u.Cout, Lo); }
-        g2_conv(u.tc, u.b, x, xu, G2Epi(), s, num_sms); launches++;
+        const GenLayer& lu = g.layers[li];
+        BV2_CHECK(lu.kind == GenLayer::UPS && lu.stage == i, "Generator plan order");
+        auto layer_of = [&](int j, int d, int c2) -> const GenLayer& { return g.layers[li + 1 + 2 * (j * nd + d) + c2]; };
+        size_t mark_after_S = 0;
+        if (!stream) {
+            const int Lo = lu.L_out;
+            t[layer_of(0, nd - 1, 1).out] = g2_h8(B, u.Cout, Lo);  // S: the next stage's input stays
+            mark_after_S = ws.used();
+            t[lu.out] = g2_h8(B, u.Cout, Lo);
+            for (int j = 0; j < nk; j++) {
+                const H8 xt = g2_h8(B, u.Cout, Lo), ra = g2_h8(B, u.Cout, Lo), rb = g2_h8(B, u.Cout, Lo);
+                for (int d = 0; d < nd; d++) {
+                    t[layer_of(j, d, 0).out] = xt;
+                    if (d < nd - 1) t[layer_of(j, d, 1).out] = d % 2 ? rb : ra;
+                }
+            }
+        }
+        conv(u.tc, u.b, G2Epi(), s);
         BV2_CUDA(cudaEventRecord(ev_fork, s));
         for (int j = 0; j < nk; j++) {
             cudaStream_t sj = j == 0 ? s : side[j];
             if (j) BV2_CUDA(cudaStreamWaitEvent(sj, ev_fork, 0));
             const ResBlockW& R = resblocks[i * nk + j];
-            H8 cur = xu;
             for (int d = 0; d < nd; d++) {
                 const bool last = d == nd - 1;
-                H8 nxt = last ? S : (cur.p == ra[j].p ? rb[j] : ra[j]);
                 G2Epi e1; e1.dil = R.dil[d];
-                g2_conv(R.c1[d].tc, R.c1[d].b, cur, xt[j], e1, sj, num_sms); launches++;
+                conv(R.c1[d].tc, R.c1[d].b, e1, sj);
                 if (last && j > 0) BV2_CUDA(cudaStreamWaitEvent(sj, ev_rb[j - 1], 0));  // S += ... after resblock j-1 wrote S
-                G2Epi e2; e2.res = &cur;
+                G2Epi e2;  // residual: the chain's input (GenLayer::res)
                 if (last) { e2.accumulate = j > 0; e2.out_scale = (j == nk - 1) ? 1.f / nk : 1.f; }
-                g2_conv(R.c2[d].tc, R.c2[d].b, xt[j], nxt, e2, sj, num_sms); launches++;
-                cur = nxt;
+                conv(R.c2[d].tc, R.c2[d].b, e2, sj);
             }
             BV2_CUDA(cudaEventRecord(ev_rb[j], sj));
         }
         if (nk > 1) BV2_CUDA(cudaStreamWaitEvent(s, ev_rb[nk - 1], 0));
-        x = S; L = Lo; ch = u.Cout;
-        ws.release(mark_after_S);
+        if (!stream) ws.release(mark_after_S);
     }
-    BV2_CHECK(ch == 16, "conv_post kernel instantiated for 16 input channels");
-    launch_pdl(k_conv_post_tanh_h8<16, 7>, dim3(cdiv(L, 512), B), dim3(256), 0, s, (const uint4*)x.p, x.Tp, conv_post_h, o, L);
-    launches++;
+    const GenLayer& lp = g.layers[li];
+    BV2_CHECK(lp.kind == GenLayer::CONV_POST && li + 1 == (int)g.layers.size(), "Generator plan order");
+    const H8& x = t[lp.in];
+    BV2_CHECK(x.C == 16, "conv_post kernel instantiated for 16 input channels");
+    const GenWin& wp = w[li];
+    if (wp.t_end > wp.t_begin) {
+        launch_pdl(k_conv_post_tanh_h8<16, 7>, dim3(cdiv(wp.t_end - wp.t_begin, 512), B), dim3(256), 0, s, (const uint4*)x.p, x.Tp, conv_post_h, o,
+                   lp.L_out, wp.t_begin, wp.t_end);
+        launches++;
+    }
 }
 
 // ================================================================================================
@@ -1231,7 +1372,7 @@ int bv2_infer_begin(bv2_engine* e, int B, int T, const int64_t* x, const int64_t
     const int H = c.hidden_channels, I = c.inter_channels;
     e->dbg.clear();
     e->ws.ensure(ws_bytes_for(c, B, T, 0));
-    e->ws.reset();
+    e->ws_reset();
     e->persist.ensure(persist_bytes_for(c, B, T, e->gproj_n));
     e->persist.reset();
     auto& st = e->st;
@@ -1275,8 +1416,9 @@ int bv2_infer_begin(bv2_engine* e, int B, int T, const int64_t* x, const int64_t
     BV2_API_END(e)
 }
 
+// open_stream: stop after the flow and open a Generator stream over o instead of running the Generator (bv2_infer_finish_stream)
 static int infer_finish_impl(bv2_engine* e, const float* noise_z, int64_t noise_ld, float noise_scale, int32_t max_len, float* o, int16_t* o16,
-                             float* attn, float* y_mask, float* z_out, float* z_p, float* m_p, float* logs_p, void* stream) {
+                             float* attn, float* y_mask, float* z_out, float* z_p, float* m_p, float* logs_p, void* stream, bool open_stream = false) {
     BV2_API_BEGIN(e)
     auto& st = e->st;
     BV2_CHECK(st.active, "infer_finish without infer_begin");
@@ -1284,8 +1426,9 @@ static int infer_finish_impl(bv2_engine* e, const float* noise_z, int64_t noise_
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const bv2_config& c = e->cfg;
     const int B = st.B, T = st.T, F = st.F, I = c.inter_channels;
-    e->ws.ensure(ws_bytes_for(c, B, T, F));
-    e->ws.reset();
+    const int Fg = (max_len > 0 && max_len < F) ? max_len : F;
+    e->ws.ensure(ws_bytes_for(c, B, T, F) + (open_stream ? e->gen_stream_bytes(B, Fg) : 0));
+    e->ws_reset();
     float* m_tmp = m_p ? m_p : e->ws.alloc((size_t)B * I * F);
     float* l_tmp = logs_p ? logs_p : e->ws.alloc((size_t)B * I * F);
     float* zp_tmp = z_p ? z_p : e->ws.alloc((size_t)B * I * F);
@@ -1309,13 +1452,16 @@ static int infer_finish_impl(bv2_engine* e, const float* noise_z, int64_t noise_
         k_c4_to_plain<<<bv2_engine::grid_tcb(F, I, B), 128, 0, s>>>(z.p, I, 0, F, z_out, I, F);
         BV2_CUDA(cudaGetLastError()); e->launches++;
     }
-    int Fg = F;
     Act zg = z;
-    if (max_len > 0 && max_len < F) {
-        Fg = max_len;
+    if (Fg < F) {
         zg = e->ws.act(B, I, Fg);
         // slice [:, :, :max_len] (reference models.py:1073): c4 rows are contiguous per (b, cg)
         BV2_CUDA(cudaMemcpy2DAsync(zg.p, (size_t)Fg * 16, z.p, (size_t)F * 16, (size_t)Fg * 16, (size_t)B * I / 4, cudaMemcpyDeviceToDevice, s));
+    }
+    if (open_stream) {
+        e->gen_stream_open(zg, st.ylen32, st.gproj + e->goff_dec, e->gproj_n, o, s);
+        st.active = false; st.finished = true;
+        return BV2_OK;
     }
     e->stage_begin("generator", s);
     if (o16) {
@@ -1347,6 +1493,28 @@ int bv2_infer_finish_pcm16(bv2_engine* e, const float* noise_z, int64_t noise_ld
     return infer_finish_impl(e, noise_z, noise_ld, noise_scale, max_len, nullptr, o16, attn, y_mask, z_out, z_p, m_p, logs_p, stream);
 }
 
+int bv2_infer_finish_stream(bv2_engine* e, const float* noise_z, int64_t noise_ld, float noise_scale, int32_t max_len, float* o,
+                            float* attn, float* y_mask, float* z_out, float* z_p, float* m_p, float* logs_p, void* stream) {
+    if (!o) return BV2_ERR_ARG;
+    return infer_finish_impl(e, noise_z, noise_ld, noise_scale, max_len, o, nullptr, attn, y_mask, z_out, z_p, m_p, logs_p, stream, true);
+}
+
+int bv2_stream_advance(bv2_engine* e, int32_t frames, void* stream, int64_t* samples_ready) {
+    BV2_API_BEGIN(e)
+    auto& gs = e->gs;
+    if (!gs.open) throw Error(BV2_ERR_STATE, "stream_advance without an open stream");
+    if (frames <= gs.frontier) throw Error(BV2_ERR_STATE, "stream_advance: frames must exceed the frames already final");
+    const int f = std::min<int>(frames, gs.Fg);
+    const std::vector<GenWin> w = gen_stream_plan(gs.g, gs.Fg, gs.frontier, f);
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (e->use_g2) e->g2_windows(gs.g, w, gs.t, true, gs.gdec, gs.g_stride, gs.o, s);
+    else e->gen_windows(gs.g, w, gs.a, true, gs.lens, gs.gdec, gs.g_stride, gs.o, s);
+    gs.frontier = f;
+    if (samples_ready) *samples_ready = (int64_t)f * e->hop;
+    if (f == gs.Fg) gs.open = false;
+    BV2_API_END(e)
+}
+
 int bv2_attn_path(bv2_engine* e, float* attn, void* stream) {
     BV2_API_BEGIN(e)
     auto& st = e->st;
@@ -1373,8 +1541,11 @@ int bv2_reserve(bv2_engine* e, int B, int T, int F_cap) {
     BV2_API_BEGIN(e)
     BV2_CHECK(e->finalized && B >= 1 && T >= 1 && F_cap >= 1, "reserve args");
     const bv2_config& c = e->cfg;
-    e->ws.ensure(ws_bytes_for(c, B, T, F_cap));
-    e->persist.ensure(persist_bytes_for(c, B, T, e->gproj_n));
+    const size_t need = ws_bytes_for(c, B, T, F_cap);
+    const size_t pneed = persist_bytes_for(c, B, T, e->gproj_n);
+    if (need > e->ws.cap() || pneed > e->persist.cap()) e->gs.open = false;  // regrowing an arena frees what an open stream reads
+    e->ws.ensure(need);
+    e->persist.ensure(pneed);
     BV2_API_END(e)
 }
 
@@ -1389,7 +1560,7 @@ int bv2_text_encoder(bv2_engine* e, int B, int T, const int64_t* x, const int64_
     BV2_CHECK(B >= 1 && B <= 4096 && T >= 1 && x && x_lengths && sid && tone && language && bert && ja_bert && en_bert && x_out && m_out && logs_out,
               "text_encoder args");
     e->dbg.clear(); e->st.active = false;
-    e->ws.ensure(ws_bytes_for(c, B, T, 0)); e->ws.reset();
+    e->ws.ensure(ws_bytes_for(c, B, T, 0)); e->ws_reset();
     e->validate_sync(B, T, x, tone, language, sid, x_lengths, s);
     int* lens = e->lens_to_device(x_lengths, B, e->ws, s);
     float* g = e->ws.alloc((size_t)B * c.gin_channels);
@@ -1415,7 +1586,7 @@ int bv2_duration(bv2_engine* e, int B, int T, const float* x, const int64_t* x_l
     const int H = c.hidden_channels;
     BV2_CHECK(B >= 1 && B <= 4096 && T >= 1 && x && x_lengths && sid && noise_w && logw_sdp && logw_dp, "duration args");
     e->dbg.clear(); e->st.active = false;
-    e->ws.ensure(ws_bytes_for(c, B, T, 0)); e->ws.reset();
+    e->ws.ensure(ws_bytes_for(c, B, T, 0)); e->ws_reset();
     e->validate_sync(B, T, nullptr, nullptr, nullptr, sid, x_lengths, s);
     int* lens = e->lens_to_device(x_lengths, B, e->ws, s);
     float* g = e->ws.alloc((size_t)B * c.gin_channels);
@@ -1447,7 +1618,7 @@ int bv2_flow_reverse(bv2_engine* e, int B, int F, const float* z_p, const int64_
     const int I = c.inter_channels;
     BV2_CHECK(B >= 1 && B <= 4096 && F >= 1 && z_p && y_lengths && sid && z_out, "flow_reverse args");
     e->dbg.clear(); e->st.active = false;
-    e->ws.ensure(ws_bytes_for(c, B, 1, F)); e->ws.reset();
+    e->ws.ensure(ws_bytes_for(c, B, 1, F)); e->ws_reset();
     e->validate_sync(B, F, nullptr, nullptr, nullptr, sid, y_lengths, s);
     int* lens = e->lens_to_device(y_lengths, B, e->ws, s);
     float* g = e->ws.alloc((size_t)B * c.gin_channels);
@@ -1472,7 +1643,7 @@ int bv2_generator(bv2_engine* e, int B, int F, const float* z_in, const float* g
     const bv2_config& c = e->cfg;
     const int I = c.inter_channels;
     e->dbg.clear(); e->st.active = false;
-    e->ws.ensure(ws_bytes_for(c, B, 1, F)); e->ws.reset();
+    e->ws.ensure(ws_bytes_for(c, B, 1, F)); e->ws_reset();
     float* gp = e->ws.alloc((size_t)B * e->gproj_n);
     e->run_gproj(g, B, gp, s);
     Act z = e->ws.act(B, I, F);

@@ -56,6 +56,7 @@ struct ConvArgs {
     float* y = nullptr;  // c4 [B][Cout_total/4][T][4]
     int Cout_total = 0, cout_off = 0, Cout = 0;
     int T = 0, B = 0;
+    int t_begin = 0, t_end = -1;  // output rows [t_begin, t_end) are computed and stored (t_end = -1: all T); reads still see all T rows
     int K = 1, dil = 1, pad = 0;
     float in_slope = 1.f;  // leaky-relu on the input (1 = identity)
     int in_mask = 0;       // input *= (t < lens[b])
@@ -85,8 +86,8 @@ __global__ void __launch_bounds__(16 * CGN * KS) k_conv1d_c4(ConvArgs a) {
     __shared__ __align__(16) float sw[CIT][K][COT];
     __shared__ __align__(16) float sred[KS > 1 ? KS : 1][KS > 1 ? NT1 : 1][4];
     const int tid = threadIdx.x % NT1, ks = threadIdx.x / NT1, tl = tid & 15, cgo = tid >> 4;
-    const int b = blockIdx.z, t0 = blockIdx.x * TT, co0 = blockIdx.y * COT;
-    const int len = a.lens ? a.lens[b] : a.T;
+    const int b = blockIdx.z, t0 = a.t_begin + blockIdx.x * TT, co0 = blockIdx.y * COT;
+    const int len = a.lens ? a.lens[b] : a.T, t_end = a.t_end < 0 ? a.T : a.t_end;
     const int xw = TT + (K - 1) * a.dil;
     float acc[NI][4];
 #pragma unroll
@@ -161,7 +162,7 @@ __global__ void __launch_bounds__(16 * CGN * KS) k_conv1d_c4(ConvArgs a) {
 #pragma unroll
     for (int i = 0; i < NI; i++) {
         int t = t0 + tl + 16 * i;
-        if (t >= a.T) continue;
+        if (t >= t_end) continue;  // stores, residual and accumulate reads stay inside the window
         float4 v = make_float4(acc[i][0] + bz.x, acc[i][1] + bz.y, acc[i][2] + bz.z, acc[i][3] + bz.w);
         if (a.act == 1) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
         if (a.res_mode) {
@@ -177,20 +178,24 @@ __global__ void __launch_bounds__(16 * CGN * KS) k_conv1d_c4(ConvArgs a) {
     }
 }
 
+// The tile shape (and with it the split of the channel reduction) is chosen for the whole length a.T, so a windowed launch keeps the
+// reduction order of every output; only the tiles covering the window are launched.
 template <int K>
 inline void launch_conv1d_k(const ConvArgs& a, cudaStream_t st) {
     const long long big_ctas = (long long)cdiv(a.T, 128) * cdiv(a.Cout, 64) * a.B;
+    const int rows = (a.t_end < 0 ? a.T : a.t_end) - a.t_begin;
     if (big_ctas >= 96) {
-        dim3 grid(cdiv(a.T, 128), cdiv(a.Cout, 64), a.B);
+        dim3 grid(cdiv(rows, 128), cdiv(a.Cout, 64), a.B);
         launch_pdl(k_conv1d_c4<K, 8, 16, 8>, grid, dim3(256), 0, st, a);
     } else {
-        dim3 grid(cdiv(a.T, 16), cdiv(a.Cout, 16), a.B);
+        dim3 grid(cdiv(rows, 16), cdiv(a.Cout, 16), a.B);
         launch_pdl(k_conv1d_c4<K, 1, 4, 32, 4>, grid, dim3(256), 0, st, a);
     }
 }
 
 inline void launch_conv1d(const ConvArgs& a, cudaStream_t st) {
     BV2_CHECK(a.dil <= 5 && a.Cin % 4 == 0 && a.Cout % 4 == 0 && a.cin_off % 4 == 0 && a.cout_off % 4 == 0, "conv1d shape");
+    BV2_CHECK(0 <= a.t_begin && a.t_begin < (a.t_end < 0 ? a.T : a.t_end) && a.t_end <= a.T, "conv1d output window");
     switch (a.K) {
         case 1: launch_conv1d_k<1>(a, st); break;
         case 3: launch_conv1d_k<3>(a, st); break;
@@ -213,6 +218,7 @@ struct ConvTArgs {
     float* y; int Cout, Tout;
     int K, u, p, B;
     float in_slope;
+    int n_begin = 0, n_end = -1;  // output samples [n_begin, n_end) are computed and stored (n_end = -1: all Tout)
 };
 
 __global__ void __launch_bounds__(256) k_convT_c4(ConvTArgs a) {
@@ -220,7 +226,8 @@ __global__ void __launch_bounds__(256) k_convT_c4(ConvTArgs a) {
     __shared__ float sx[CIT][XW];
     __shared__ __align__(16) float sw[CIT][KMAX][COT];
     const int tid = threadIdx.x, tl = tid & 15, cgo = tid >> 4;
-    const int b = blockIdx.z, n0 = blockIdx.x * TT, co0 = blockIdx.y * COT;
+    const int b = blockIdx.z, n0 = a.n_begin + blockIdx.x * TT, co0 = blockIdx.y * COT;
+    const int n_end = a.n_end < 0 ? a.Tout : a.n_end;
     const int taps = a.K / a.u;
     const int i_base = (n0 + a.p) / a.u - (taps - 1);
     const int xw = (TT - 1 + a.p + n0) / a.u - i_base + 1;  // <= TT/u + taps
@@ -278,7 +285,7 @@ __global__ void __launch_bounds__(256) k_convT_c4(ConvTArgs a) {
 #pragma unroll
     for (int i = 0; i < 8; i++) {
         int n = n0 + tl + 16 * i;
-        if (n < a.Tout) y4[n] = make_float4(acc[i][0] + bz.x, acc[i][1] + bz.y, acc[i][2] + bz.z, acc[i][3] + bz.w);
+        if (n < n_end) y4[n] = make_float4(acc[i][0] + bz.x, acc[i][1] + bz.y, acc[i][2] + bz.z, acc[i][3] + bz.w);
     }
 }
 
@@ -902,13 +909,13 @@ __global__ void k_flip_c4(const float* __restrict__ x, float* __restrict__ y, in
 // ------------------------------------------------------------------------------------------------
 template <int C, int K>
 __global__ void __launch_bounds__(256) k_conv_post_tanh(const float* __restrict__ x, const float* __restrict__ w,
-                                                       float* __restrict__ y, int T, float slope) {
+                                                       float* __restrict__ y, int T, float slope, int t_begin, int t_end) {
     __shared__ float sw[C * K];
     for (int i = threadIdx.x; i < C * K; i += blockDim.x) sw[i] = w[i];  // [C][K]
     __syncthreads();
-    int t = blockIdx.x * blockDim.x + threadIdx.x;
+    int t = t_begin + blockIdx.x * blockDim.x + threadIdx.x;  // outputs [t_begin, t_end) of T
     int b = blockIdx.y;
-    if (t >= T) return;
+    if (t >= t_end) return;
     const float4* x4 = reinterpret_cast<const float4*>(x) + (size_t)b * (C / 4) * T;
     float acc = 0.f;
 #pragma unroll

@@ -53,6 +53,7 @@ struct TcEpi {
     int bias_b_stride = 0;
     int cin_off = 0, cout_off = 0;  // channel windows inside x / y (multiples of 4; of 8 for 16-bit tensors)
     int dil = 1;
+    int t_begin = 0, t_end = -1;  // output window [t_begin, t_end) (t_end = -1: the whole output); a ConvTranspose window is a multiple of its stride
     int out_tf32 = 0;    // round the stored output to TF32 (RN): a TF32 consumer may then skip its operand prologue
     int skip_xform = 0;  // TF32: input already TF32-exact, no activation / mask / padding needed (K == 1)
     int in_f16 = 0;      // FP16: x is a 16-bit c8 tensor [B][C/8][T][8] (the operand image itself: no prologue; K == 1)
@@ -136,13 +137,18 @@ inline TcConvW tc_pack_weights(std::function<float*(const std::vector<float>&)>&
 //   out[t*u + r][co] = sum_m sum_ci x[t + floor((r+p)/u) - m][ci] * w[ci][co][(r+p)%u + m*u]
 // -> an ordinary conv over input-rate time with Kp taps (union of the per-phase offsets), N = u*Cout columns ordered
 // (r, co), structural zeros where a phase does not use a tap.  wT: [Cin][Cout][K] (weight-norm folded).
-inline TcConvW tc_pack_upsample(std::function<float*(const std::vector<float>&)>& up, const std::vector<float>& wT, int Cin, int Cout, int K, int u,
-                                int kc = 0, int f16 = 0, bool fill = true, int nt_max = 128) {
+// Input rows t - half .. t + half feed the u outputs of input row t of the polyphase ConvTranspose1d (stride u, K taps, padding (K-u)/2).
+inline int ups_half(int K, int u) {
     const int p = (K - u) / 2, taps = K / u;
     int omin = 1 << 30, omax = -(1 << 30);
     for (int r = 0; r < u; r++)
         for (int m = 0; m < taps; m++) { int o = (r + p) / u - m; omin = std::min(omin, o); omax = std::max(omax, o); }
-    int half = std::max(-omin, omax);
+    return std::max(-omin, omax);
+}
+inline TcConvW tc_pack_upsample(std::function<float*(const std::vector<float>&)>& up, const std::vector<float>& wT, int Cin, int Cout, int K, int u,
+                                int kc = 0, int f16 = 0, bool fill = true, int nt_max = 128) {
+    const int p = (K - u) / 2, taps = K / u;
+    const int half = ups_half(K, u);
     const int Kp = 2 * half + 1;  // symmetric so that pad = (Kp-1)/2
     std::vector<float> w((size_t)u * Cout * Cin * Kp, 0.f);  // [N = u*Cout][Cin][Kp]
     for (int r = 0; fill && r < u; r++)
@@ -163,6 +169,7 @@ struct TcParams {
     int Cin_total, cin_off, Cout_total, cout_off, res_C_total, res_c_off, bias_b_stride;
     int nt;           // columns per N tile
     int T, B, K, dil, pad, KC, nchunks, R, nws, nas, MT;
+    int t_begin, t_end;  // rows [t_begin, t_end) of the M axis (output time; input time of a ConvTranspose) are stored; t_end = 0: all T rows
     uint32_t a_stage_bytes, a_op_off, w_stage_bytes, acc_cols;  // acc_cols: columns of the accumulator image
     float in_slope, out_scale;
     int accumulate, relu, res_mode, in_mask, out_mask, ups_u, ups_cout;
@@ -353,6 +360,8 @@ __device__ __forceinline__ uint32_t pack_h2(float lo, float hi) {
     return r;
 }
 
+__device__ __forceinline__ int tc_t_end(const TcParams& p) { return p.t_end > 0 ? p.t_end : p.T; }
+
 // Pre-load one 128-row x nt accumulator tile: bias (+ per-batch bias) (+/- residual) (+ previous output).
 // All global loads of a 32-column batch are issued before the first image stores (memory-level parallelism: the
 // epilogue warps are the only threads touching residual/output tensors).
@@ -360,7 +369,7 @@ __device__ __forceinline__ uint32_t pack_h2(float lo, float hi) {
 // epilogue.  The plain instantiation keeps the MRF convs (most of the launches) free of the generic tail's registers and branches.
 template <int NG, int GEN>
 __device__ __forceinline__ void acc_init_tile(const TcParams& p, uint32_t trow, int b, int t, int n0, int nt, int yb = -1, int coff = -1, bool skip_res = false) {
-    const bool ok = t < p.T;
+    const bool ok = t < tc_t_end(p);  // stores, residual reads and accumulate reads stay inside the window
     const size_t tstride = (size_t)p.T * ((GEN && p.ups_u) ? p.ups_u : 1);
     if (yb < 0) yb = b;
     if (coff < 0) coff = p.cout_off;
@@ -416,7 +425,7 @@ __device__ __forceinline__ void acc_init_tile(const TcParams& p, uint32_t trow, 
 // Drain one accumulator tile: the accumulator image -> [relu] -> scale/mask -> c4 global (16-byte stores, coalesced across a warp).
 template <int NG, int GEN>
 __device__ __forceinline__ void acc_tail_tile(const TcParams& p, uint32_t trow, int b, int t, int n0, int nt, int len, int yb = -1, int coff = -1) {
-    const bool ok = t < p.T;
+    const bool ok = t < tc_t_end(p);  // stores, residual reads and accumulate reads stay inside the window
     const size_t tstride = (size_t)p.T * ((GEN && p.ups_u) ? p.ups_u : 1);
     if (yb < 0) yb = b;
     if (coff < 0) coff = p.cout_off;
@@ -484,7 +493,7 @@ __device__ __forceinline__ void acc_tail_tile(const TcParams& p, uint32_t trow, 
 __device__ __forceinline__ void acc_tail_ln(const TcParams& p, uint32_t trow, int b, int t, int nt, int len, const float4* rs = nullptr) {
     // rs: this thread's row of the TMA-staged residual tile ([nt/4][128 rows] float4, already offset by the row); nullptr = the residual
     // was pre-loaded into the accumulator.  x = acc + residual is re-formed in each pass (shared-memory reads are cheap, the accumulator image is not written).
-    const bool ok = t < p.T;
+    const bool ok = t < tc_t_end(p);  // stores, residual reads and accumulate reads stay inside the window
     float4* ybp = reinterpret_cast<float4*>(p.y) + (size_t)b * (p.Cout_total / 4) * p.T;
     float s = 0.f;
     for (int c0 = 0; c0 < nt; c0 += 32) {
@@ -613,7 +622,7 @@ __global__ void __launch_bounds__(384, 1) k_tc_conv1d(TcParams p) {
     uint8_t* smem = smem_raw + acc_img_bytes(p.acc_cols);  // behind the accumulator image
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int MT = p.MT;
-    const int t0 = blockIdx.x * 128 * MT, n0 = blockIdx.y * p.nt, z = blockIdx.z;
+    const int t0 = p.t_begin + blockIdx.x * 128 * MT, n0 = blockIdx.y * p.nt, z = blockIdx.z;
     const int zs = p.zsplit > 1 ? p.zsplit : 1;
     const int b = z / zs, hz = z - b * zs;
     const int xb = p.x_batch_z ? z : b, yb = p.y_batch_z ? z : b;
@@ -864,7 +873,7 @@ __global__ void __launch_bounds__(512, 1) k_tc_conv1d_persist(TcParams p, int mt
         asm volatile("griddepcontrol.wait;" ::: "memory");
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
         for (int i = 0; i < n_mine; i++) {
-            const int tile = blockIdx.x + i * gridDim.x, b = tile / mtiles, t0 = (tile - b * mtiles) * 128;
+            const int tile = blockIdx.x + i * gridDim.x, b = tile / mtiles, t0 = p.t_begin + (tile - b * mtiles) * 128;
             const int r_lo = max(0, p.pad - t0), r_hi = min(R, p.T - (t0 - p.pad));
             const uint32_t row_bytes = (uint32_t)(r_hi - r_lo) * 16u;
             const int sa = i % NAS;
@@ -909,7 +918,7 @@ __global__ void __launch_bounds__(512, 1) k_tc_conv1d_persist(TcParams p, int mt
         const int tid2 = threadIdx.x - 64;
         const float slope = p.in_slope;
         for (int i = 0; i < n_mine; i++) {
-            const int tile = blockIdx.x + i * gridDim.x, b = tile / mtiles, t0 = (tile - b * mtiles) * 128;
+            const int tile = blockIdx.x + i * gridDim.x, b = tile / mtiles, t0 = p.t_begin + (tile - b * mtiles) * 128;
             const int len = p.lens ? p.lens[b] : p.T;
             const int r_lo = max(0, p.pad - t0), r_hi = min(R, p.T - (t0 - p.pad));
             const int r_mask_hi = p.in_mask ? min(r_hi, len - (t0 - p.pad)) : r_hi;
@@ -927,14 +936,14 @@ __global__ void __launch_bounds__(512, 1) k_tc_conv1d_persist(TcParams p, int mt
         // ===== accumulator init (tile i+1) and tail (tile i), double-buffered accumulator image
         const int q = warp & 3;
         auto init_tile = [&](int i) {
-            const int tile = blockIdx.x + i * gridDim.x, b = tile / mtiles, t0 = (tile - b * mtiles) * 128;
+            const int tile = blockIdx.x + i * gridDim.x, b = tile / mtiles, t0 = p.t_begin + (tile - b * mtiles) * 128;
             acc_init_tile<4, GEN>(p, acc0 + ((uint32_t)(q * 32) << 16) + (uint32_t)((i & 1) * nt), b, t0 + q * 32 + lane, 0, nt);
             mbar_arrive(BAR(B_INIT + (i & 1)));
         };
         if (n_mine > 0) init_tile(0);
         for (int i = 0; i < n_mine; i++) {
             if (i + 1 < n_mine) init_tile(i + 1);
-            const int tile = blockIdx.x + i * gridDim.x, b = tile / mtiles, t0 = (tile - b * mtiles) * 128;
+            const int tile = blockIdx.x + i * gridDim.x, b = tile / mtiles, t0 = p.t_begin + (tile - b * mtiles) * 128;
             const int len = p.lens ? p.lens[b] : p.T;
             mbar_wait(BAR(B_ACC + (i & 1)), (i >> 1) & 1);
             acc_tail_tile<4, GEN>(p, acc0 + ((uint32_t)(q * 32) << 16) + (uint32_t)((i & 1) * nt), b, t0 + q * 32 + lane, 0, nt, len);
@@ -983,7 +992,7 @@ __global__ void __launch_bounds__(512, 1) k_tc_conv1d_pstream(TcParams p, int mt
         ntile = tile % ntiles;
         const int mm = tile / ntiles;
         b = mm / mtiles;
-        t0 = (mm - b * mtiles) * 128 * MT;
+        t0 = p.t_begin + (mm - b * mtiles) * 128 * MT;
     };
     (void)ncg;
 
@@ -1175,6 +1184,12 @@ inline TcConvPlan tc_conv_plan(const TcConvW& w, const float* bias, const Act& x
     p.res_C_total = e.res_C_total ? e.res_C_total : y.C; p.res_c_off = e.res_c_off; p.bias_b_stride = e.bias_b_stride;
     p.T = x.T; p.B = x.B; p.K = w.K; p.dil = e.dil; p.pad = (w.K - 1) / 2 * e.dil;
     p.KC = w.KC; p.nchunks = w.nchunks;
+    // Output window: the kernel variant and its pipeline shape are chosen for the whole length (p.T) and only the tiles covering the
+    // window are launched, so every output keeps the reduction order of the full-length launch.
+    const int t_end = e.t_end < 0 ? y.T : e.t_end;
+    BV2_CHECK(0 <= e.t_begin && e.t_begin < t_end && t_end <= y.T && e.t_begin % u == 0 && t_end % u == 0, "tc_conv1d output window");
+    p.t_begin = e.t_begin / u; p.t_end = t_end / u;
+    const int wrows = p.t_end - p.t_begin;
     const int nt = w.nt;
     if (w.ups_u) BV2_CHECK(w.ups_cout % 4 == 0, "ups cout");
     p.nt = nt;
@@ -1211,7 +1226,7 @@ inline TcConvPlan tc_conv_plan(const TcConvW& w, const float* bias, const Act& x
         p.acc_cols = (uint32_t)(2 * nt);
         const size_t smem_p = tc::acc_img_bytes(p.acc_cols) + wb + (size_t)p.nas * p.a_stage_bytes + (size_t)(3 * p.nas + 5) * 8 + 16;
         const int per_sm = 1;  // 512 threads at > 64 registers: one CTA per SM
-        const int mtiles = cdiv(p.T, 128);
+        const int mtiles = cdiv(wrows, 128);
         const int total = mtiles * p.B;
         const int grid_p = std::min(total, per_sm * num_sms);
         pl.kind = TC_PERSIST; pl.nas = p.nas; pl.nws = 0; pl.smem = smem_p; pl.grid = dim3(grid_p); pl.block = dim3(512);
@@ -1235,7 +1250,7 @@ inline TcConvPlan tc_conv_plan(const TcConvW& w, const float* bias, const Act& x
         p.acc_cols = (uint32_t)(2 * MT * nt);
         const size_t smem_s = img + (size_t)nas2 * p.a_stage_bytes + (size_t)nws2 * p.w_stage_bytes + (size_t)(3 * nas2 + 2 * nws2 + 4) * 8 + 16;
         BV2_CHECK(smem_s <= 227 * 1024, "tc_conv1d pstream shared memory");
-        const int mtiles = cdiv(p.T, 128 * MT);
+        const int mtiles = cdiv(wrows, 128 * MT);
         const int total = mtiles * p.B * ntiles;
         const int grid_s = std::min(total, num_sms);
         pl.kind = TC_PSTREAM; pl.nas = p.nas; pl.nws = p.nws; pl.smem = smem_s; pl.grid = dim3(grid_s); pl.block = dim3(512);
@@ -1267,8 +1282,8 @@ inline TcConvPlan tc_conv_plan(const TcConvW& w, const float* bias, const Act& x
     if (res_smem) { smem = (smem + 15) & ~(size_t)15; p.res_soff = (uint32_t)(smem - img); smem += res_bytes; }  // offset from the kernel's `smem` (behind the image)
     BV2_CHECK(smem <= 227 * 1024, "tc_conv1d shared memory");
     pl.kind = TC_ONE_TILE; pl.res_smem = res_smem ? 1 : 0; pl.nas = p.nas; pl.nws = p.nws; pl.smem = smem;
-    pl.grid = dim3(cdiv(p.T, 128), ntiles, p.B); pl.block = dim3(384);
-    pl.mtiles = cdiv(p.T, 128); pl.ntiles = ntiles; pl.total = pl.mtiles * ntiles * p.B;
+    pl.grid = dim3(cdiv(wrows, 128), ntiles, p.B); pl.block = dim3(384);
+    pl.mtiles = cdiv(wrows, 128); pl.ntiles = ntiles; pl.total = pl.mtiles * ntiles * p.B;
     return pl;
 }
 

@@ -43,6 +43,7 @@ struct G2Params {
     const uint4* x; uint4* y; const uint4* res; const void* w; const float* bias; const float* bias_b;
     int x_cg, x_Tp, y_cg, y_Tp, res_cg, res_Tp, bias_b_stride;
     int T, K, dil, pad, nt, KC, nchunks, NG, MG, R, nas, nws, resident;
+    int t_begin, t_end;  // rows [t_begin, t_end) of the M axis are computed and stored (M = output time; input time of a ConvTranspose)
     uint32_t a_stage_bytes, w_stage_bytes, acc_cols;  // acc_cols: columns of the accumulator image
     int residual, accumulate, ups_u, ups_cout;
     float out_scale;
@@ -137,7 +138,7 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
     uint8_t* smem = smem_raw + acc_img_bytes(p.acc_cols);  // behind the accumulator image
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;  // shfl: warp-uniform for the compiler
     const int NAS = p.nas, NWS = p.nws, NG = p.NG, MG = p.MG, NCH = p.nchunks, nt = p.nt, R = p.R;
-    const int t0 = blockIdx.x * NG * MG * 128, ntile = blockIdx.y, n0 = ntile * nt, b = blockIdx.z;
+    const int t0 = p.t_begin + blockIdx.x * NG * MG * 128, ntile = blockIdx.y, n0 = ntile * nt, b = blockIdx.z;
     long long* prof = p.prof ? p.prof + ((size_t)(blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 16 : nullptr;
     if (prof && threadIdx.x == 0) prof[0] = gtime();
     uint8_t* sA = smem;
@@ -170,7 +171,7 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
         for (int s = 0; s < steps; s++) {
             const int g = s / NCH, c = s - g * NCH, sa = s % NAS;
             const int row0 = t0 + g * MG * 128 - p.pad;
-            const int nrows = max(0, min(R, p.T + G2_PADR - row0));  // never read past the tensor's halo; rows beyond feed discarded outputs only
+            const int nrows = max(0, min(R, p.T + G2_PADR - row0));  // never read past the tensor's halo; rows beyond (and rows past a window's end) feed discarded outputs only
             if ((p.dbg_flags & 4) && s >= NAS) continue;
             if (lane == 0) {
                 mbar_wait(BAR(B_AEMPTY + sa), ((s / NAS) & 1) ^ 1);
@@ -235,16 +236,18 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
         else g2_issuer_mg<1>(q, MG, prof, lane);  // g2_conv() admits KC = 16 or 32 only
     } else if (warp == 3) {
         // ===== zero halo of the OUTPUT tensor (= the conv padding of its consumers), written by its producer: the CTA of the first super-tile
-        // clears rows [-G2_PADL, 0), the CTA of the last one rows [T_out, T_out + G2_PADR), for every channel group of batch b (N tile 0 only).
-        // (Round 2 until now: one k_g2_zero_halo launch per Generator stage -- six plain launches, each a full drain of the PDL chain.)
-        if (!(p.dbg_flags & 16) && ntile == 0 && (blockIdx.x == 0 || blockIdx.x == gridDim.x - 1)) {
+        // clears rows [-G2_PADL, 0) if the window starts at t = 0, the CTA of the last one rows [T_out, T_out + G2_PADR) if the window ends at
+        // T_out, for every channel group of batch b (N tile 0 only).  A window inside the tensor leaves the halo rows alone: in a streamed run
+        // they are final rows of earlier windows.
+        const bool lo = blockIdx.x == 0 && p.t_begin == 0, hi = blockIdx.x == gridDim.x - 1 && p.t_end == p.T;
+        if (!(p.dbg_flags & 16) && ntile == 0 && (lo || hi)) {
             asm volatile("griddepcontrol.wait;" ::: "memory");  // the rows may alias a tensor an upstream kernel is still reading
             uint4* yb = p.y + (size_t)b * p.y_cg * p.y_Tp;
             const int Tout = p.T * (p.ups_u ? p.ups_u : 1);
             const uint4 z4 = make_uint4(0u, 0u, 0u, 0u);
-            if (blockIdx.x == 0)
+            if (lo)
                 for (int i = lane; i < p.y_cg * G2_PADL; i += 32) yb[(size_t)(i / G2_PADL) * p.y_Tp + (i % G2_PADL) - G2_PADL] = z4;
-            if (blockIdx.x == gridDim.x - 1)
+            if (hi)
                 for (int i = lane; i < p.y_cg * G2_PADR; i += 32) yb[(size_t)(i / G2_PADR) * p.y_Tp + Tout + (i % G2_PADR)] = z4;
         }
     } else if (warp >= 4 && warp < 16) {
@@ -296,7 +299,7 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
             for (int it = part; it < MG * ncb; it += 3) {
                 const int mt = it / ncb, col0 = (it - mt * ncb) * cw;
                 const int t = t0 + (g * MG + mt) * 128 + q * 32 + lane;
-                const bool ok = t < p.T;
+                const bool ok = t < p.t_end;  // stores, residual reads and running-sum updates stay inside the window
                 uint32_t v[32];
                 if (cw == 32) acc_ld<32>(trow + (uint32_t)((g * MG + mt) * nt + col0), v); else acc_ld<16>(trow + (uint32_t)((g * MG + mt) * nt + col0), v);
                 // residual / running-sum operands are fetched while the accumulator image load is in flight
@@ -386,12 +389,14 @@ __global__ void __launch_bounds__(128) k_c4_to_h8(const float4* __restrict__ x, 
 // stages TB + K - 1 rows ONCE as activated fp32 in shared memory (coalesced 16-byte loads, conflict-free stores), the weights ride in the
 // kernel parameters (constant bank: FFMA takes them as an operand), and a thread's inner loop is one conflict-free LDS + one FFMA per tap.
 template <int C, int K> struct PostW { float w[C * K]; };  // [C][K]
+// Outputs [t_begin, t_end) of the T samples are stored; staged rows past t_end feed discarded outputs only.
 template <int C, int K>
-__global__ void __launch_bounds__(256) k_conv_post_tanh_h8(const uint4* __restrict__ x, int Tp, const __grid_constant__ PostW<C, K> pw, float* __restrict__ y, int T) {
+__global__ void __launch_bounds__(256) k_conv_post_tanh_h8(const uint4* __restrict__ x, int Tp, const __grid_constant__ PostW<C, K> pw, float* __restrict__ y, int T,
+                                                           int t_begin, int t_end) {
     constexpr int TB = 512, RW = TB + K - 1, LD = RW + 2;  // outputs per block, staged rows, row stride of the staged tile
     __shared__ float sx[C][LD];
     asm volatile("griddepcontrol.wait;" ::: "memory");
-    const int t0 = blockIdx.x * TB, b = blockIdx.y;
+    const int t0 = t_begin + blockIdx.x * TB, b = blockIdx.y;
     for (int i = threadIdx.x; i < (C / 8) * RW; i += blockDim.x) {
         const int g = i / RW, r = i - g * RW, row = t0 - K / 2 + r;  // row >= -K/2 >= -G2_PADL; rows >= T + G2_PADR lie outside the allocation
         float f[8];
@@ -416,7 +421,7 @@ __global__ void __launch_bounds__(256) k_conv_post_tanh_h8(const uint4* __restri
                 for (int k = 0; k < 8; k++) acc = fmaf(sx[g * 8 + k][tl + j], pw.w[(g * 8 + k) * K + j], acc);
             }
         }
-        if (t < T) y[(size_t)b * T + t] = tanhf(acc);
+        if (t < t_end) y[(size_t)b * T + t] = tanhf(acc);
     }
 }
 
@@ -430,6 +435,7 @@ struct G2Epi {
     float out_scale = 1.f;
     const float* bias_b = nullptr; int bias_b_stride = 0;  // per-batch bias (speaker conditioning of conv_pre)
     int dil = 1;
+    int t_begin = 0, t_end = -1;  // output window [t_begin, t_end) (t_end = -1: T_out); a ConvTranspose window is a multiple of its stride
     int st_override = 0;      // probes: force the super-tile size (m-tiles per CTA)
     long long* prof = nullptr;  // probes: per-CTA timestamps
     int dbg_skip_wcommit = 0;
@@ -465,10 +471,14 @@ inline G2Plan g2_conv_plan(const TcConvW& w, const float* bias, const H8& x, con
     p.T = x.T; p.K = w.K; p.dil = e.dil; p.pad = (w.K - 1) / 2 * e.dil;
     BV2_CHECK(p.pad <= G2_PADL && p.pad <= G2_PADR, "g2_conv padding exceeds the tensor halo");
     p.nt = w.nt; p.KC = w.KC; p.nchunks = w.nchunks;
+    const int t_end = e.t_end < 0 ? y.T : e.t_end;
+    BV2_CHECK(0 <= e.t_begin && e.t_begin < t_end && t_end <= y.T && e.t_begin % u == 0 && t_end % u == 0, "g2_conv output window");
+    p.t_begin = e.t_begin / u; p.t_end = t_end / u;
     const int ntiles = w.Cout / w.nt, halo = (w.K - 1) * e.dil;
     p.w_stage_bytes = (uint32_t)(w.KC * w.nt * 2);
-    // the accumulator image of a CTA holds at most 128 columns of 128 rows (66 KB of shared memory)
-    const int mtiles = cdiv(x.T, 128), mgmax = std::max(1, 128 / w.nt);
+    // the accumulator image of a CTA holds at most 128 columns of 128 rows (66 KB of shared memory).  The time tiling follows the window;
+    // the reduction order of every output (bias, then chunk c, tap j, k-step) does not depend on it.
+    const int mtiles = cdiv(p.t_end - p.t_begin, 128), mgmax = std::max(1, 128 / w.nt);
     const size_t img = tc::acc_img_bytes((uint32_t)(mgmax * w.nt)), budget = 220 * 1024 - img;
     const size_t w_all = (size_t)w.nchunks * w.K * p.w_stage_bytes;
     p.resident = w_all <= 48 * 1024 && ntiles == 1;

@@ -171,6 +171,33 @@ class Engine:
                 _ptr(attn), _ptr(y_mask), _ptr(z), _ptr(z_p), _ptr(m_p), _ptr(logs_p), self._stream()))
         return o, attn, y_mask, (z, z_p, m_p, logs_p)
 
+    def infer_finish_stream(self, B, T, F, noise_z, noise_scale, max_len=None, want_attn=True):
+        """infer_finish up to and including the flow, then open a Generator stream over the returned `o` [B,1,Fg*hop]; its samples become
+        final as stream_advance() is called.  Returns (o, attn, y_mask, (z, z_p, m_p, logs_p)) like infer_finish.  Every precision;
+        no pcm16 (its peak normalisation needs the whole utterance)."""
+        I, hop = self.cfg.inter_channels, self.cfg.hop
+        noise_z = self._f32(noise_z)
+        assert noise_z.shape[0] == B and noise_z.shape[1] == I and noise_z.shape[2] >= F
+        Fg = F if (max_len is None or max_len >= F) else int(max_len)
+        dev = self.device
+        o = torch.empty(B, 1, Fg * hop, device=dev, dtype=torch.float32)
+        attn = torch.empty(B, 1, F, T, device=dev, dtype=torch.float32) if want_attn else None
+        y_mask = torch.empty(B, 1, F, device=dev, dtype=torch.float32)
+        z, z_p, m_p, logs_p = (torch.empty(B, I, F, device=dev, dtype=torch.float32) for _ in range(4))
+        self._last = (B, T, F)
+        self._check(self.lib.bv2_infer_finish_stream(self._h, _ptr(noise_z), noise_z.shape[2], float(noise_scale),
+                                                     -1 if max_len is None else int(max_len), _ptr(o), _ptr(attn), _ptr(y_mask), _ptr(z),
+                                                     _ptr(z_p), _ptr(m_p), _ptr(logs_p), self._stream()))
+        self._stream_o = o  # the stream writes into o until it closes
+        return o, attn, y_mask, (z, z_p, m_p, logs_p)
+
+    def stream_advance(self, frames: int) -> int:
+        """Enqueue the Generator work that makes o[..., :min(frames, Fg)*hop] final on the current stream; returns that sample count.
+        Raises Bv2Error if no stream is open or `frames` does not exceed the frames already final."""
+        n = C.c_int64(0)
+        self._check(self.lib.bv2_stream_advance(self._h, int(frames), self._stream(), C.byref(n)))
+        return int(n.value)
+
     def attn_path(self) -> torch.Tensor:
         """attn [B,1,F,T] of the last infer_begin/infer_finish, materialised on demand (valid until the next infer_begin)."""
         B, T, F = self._last

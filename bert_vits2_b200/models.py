@@ -163,5 +163,45 @@ class SynthesizerTrn(nn.Module):
         self.last_y_lengths = y_lengths
         return o, LazyAttn(eng, (B, 1, F, T), token), y_mask, aux
 
+    @torch.no_grad()
+    def infer_stream(self, x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_scale=0.667, length_scale=1,
+                     noise_scale_w=0.8, max_len=None, sdp_ratio=0, y=None, *, noise_w=None, noise_z=None, w_ceil_override=None,
+                     first_chunk_frames=32):
+        """Streaming infer(): a generator of waveform chunks o[:, :, a:b] (device tensors, views of one [B,1,Fg*hop] buffer) whose
+        concatenation is bit-identical to infer(...)[0] with the same noise.  Encoder, durations and flow run whole first (the flow's
+        attention spans the utterance); the Generator then runs as a wavefront, so the first chunk costs about first_chunk_frames
+        + 14 frames of Generator work instead of all of it.  Chunks are first_chunk_frames frames, then double.  Each chunk is final
+        when it is yielded (the host waits on an event recorded after its work) and no later chunk writes it.  Noise is drawn exactly
+        as infer() draws it.  `last_y_lengths` is set before the first chunk.  There is no pcm16 option: the PCM conversion normalises by the peak of the whole utterance."""
+        dev = next(self.parameters()).device
+        if dev.type != "cuda":
+            raise Bv2Error("SynthesizerTrn.infer_stream: module is on CPU; bert_vits2_b200 has no CPU path — call .to('cuda')")
+        if x.dim() != 2 or bert.dim() != 3 or bert.shape[-1] != x.shape[1]:
+            raise ValueError("expected x [B,T] and bert features [B,1024,T]")
+        if first_chunk_frames < 1:
+            raise ValueError("first_chunk_frames must be >= 1")
+        eng = self._engine(dev)
+        B, T = x.shape
+        if noise_w is None:
+            noise_w = torch.randn(B, 2, T, device=dev, dtype=torch.float32)
+        y_lengths, F = eng.infer_begin(x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_w, noise_scale_w,
+                                       length_scale, sdp_ratio, w_ceil_override)
+        if noise_z is None:
+            noise_z = torch.randn(B, self.inter_channels, F, device=dev, dtype=torch.float32)
+        o, _, _, _ = eng.infer_finish_stream(B, T, F, noise_z, noise_scale, max_len, want_attn=False)
+        eng._attn_token = object()  # a LazyAttn of an earlier infer() must not materialise this utterance's path
+        self.last_y_lengths = y_lengths
+        hop = self.cfg.hop
+        Fg = o.shape[-1] // hop
+        done, step = 0, int(first_chunk_frames)
+        while done < Fg:
+            target = min(done + step, Fg)
+            eng.stream_advance(target)
+            ev = torch.cuda.Event()
+            ev.record(torch.cuda.current_stream(dev))
+            ev.synchronize()
+            yield o[:, :, done * hop:target * hop]
+            done, step = target, 2 * step
+
     def forward(self, *a, **kw):
         raise NotImplementedError("training forward (reference models.py:937-1024) is out of scope; use .infer()")

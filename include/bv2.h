@@ -101,6 +101,22 @@ int bv2_infer_finish(bv2_engine* e, const float* noise_z, int64_t noise_ld, floa
 int bv2_infer_finish_pcm16(bv2_engine* e, const float* noise_z, int64_t noise_ld, float noise_scale, int32_t max_len,
                            int16_t* o16, float* attn, float* y_mask, float* z, float* z_p, float* m_p, float* logs_p,
                            void* stream);
+/* Streaming synthesis: audio leaves the Generator in chunks, before the whole utterance has gone through it.
+ * bv2_infer_finish_stream does what bv2_infer_finish does up to and including the flow (same arguments and outputs), then opens a
+ * stream over the caller's o [B,1,Fg*hop], which must stay allocated until the stream is closed.  Every
+ * generator_precision streams.
+ * bv2_stream_advance enqueues on `stream` the Generator work that makes o[..., :min(frames, Fg)*hop] final and writes that sample count
+ * to *samples_ready (HOST, may be NULL).  Each layer computes a time window of its output as soon as its input is final far enough
+ * ahead (every output element exactly once), so the streamed o is bit-identical to the one bv2_infer_finish writes.  The stream
+ * closes when it reaches Fg.  frames not above the frames already final, or an advance without an open stream, return
+ * BV2_ERR_STATE.  Every call that resets the workspace (bv2_infer_begin, bv2_infer_finish*, the per-stage entry points, a growing
+ * bv2_reserve) closes an open stream.  A stream keeps all Generator activations alive: about 1.19 MB (FP16 Generator) or 2.37 MB (fp32 /
+ * TF32) per frame per utterance at the default configuration (engine.cu states the exact figures).  16-bit PCM is not streamed: its peak normalisation needs the whole
+ * utterance. */
+int bv2_infer_finish_stream(bv2_engine* e, const float* noise_z, int64_t noise_ld, float noise_scale, int32_t max_len,
+                            float* o, float* attn, float* y_mask, float* z, float* z_p, float* m_p, float* logs_p, void* stream);
+int bv2_stream_advance(bv2_engine* e, int32_t frames, void* stream, int64_t* samples_ready);
+
 /* The same conversion for a waveform batch the caller already holds: wave [B,L] fp32 (device), n_valid [B] int64 (device,
  * may be NULL = L) -> out [B,L] int16 (device). */
 int bv2_wave_to_pcm16(bv2_engine* e, int B, int64_t L, const float* wave, const int64_t* n_valid, int16_t* out, void* stream);
