@@ -10,7 +10,6 @@ import threading
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 LIB_PATH = os.path.join(HERE, "libbv2.so")
-TUNING_LIB_PATH = os.path.join(HERE, "libbv2_tuning.so")  # development build (-DBV2_TUNING: the BV2_* environment knobs of the probes are live)
 SOURCES = [os.path.join(HERE, "csrc", "engine.cu")]
 HEADERS = sorted(os.path.join(HERE, "csrc", f) for f in os.listdir(os.path.join(HERE, "csrc")) if f.endswith(".cuh")) + [
     os.path.join(ROOT, "include", "bv2.h")]
@@ -86,26 +85,22 @@ def needs_build() -> bool:
     return any(os.path.getmtime(p) > t for p in SOURCES + HEADERS if os.path.isfile(p))
 
 
-def build(force: bool = False, verbose: bool = False, tuning: bool = False) -> str:
-    """Compile libbv2.so in-tree for sm_90a with nvcc (cross-compiles without a GPU).
-    tuning=True builds libbv2_tuning.so instead (same sources, -DBV2_TUNING); it is only ever loaded when BV2_LIB points at it."""
+def build(force: bool = False, verbose: bool = False) -> str:
+    """Compile libbv2.so in-tree for sm_90a with nvcc (cross-compiles without a GPU)."""
     with _lock:
-        out = TUNING_LIB_PATH if tuning else LIB_PATH
-        if not tuning and not force and not needs_build():
+        if not force and not needs_build():
             return LIB_PATH
-        tmp = out + ".tmp"  # link to a temporary name, then rename: a reader never sees a half-written library
+        tmp = LIB_PATH + ".tmp"  # link to a temporary name, then rename: a reader never sees a half-written library
         cmd = ["nvcc"] + NVCC_FLAGS + ["-o", tmp] + SOURCES
-        if tuning or os.environ.get("BV2_BUILD_TUNING"):  # development builds: BV2_* environment knobs of the probes become active (tc_conv.cuh tune_env)
-            cmd.insert(1, "-DBV2_TUNING")
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("nvcc failed:\n" + r.stdout + r.stderr)
-        os.replace(tmp, out)
+        os.replace(tmp, LIB_PATH)
         if verbose:
             print(r.stderr)
-        return out
+        return LIB_PATH
 
 
 def harness_needs_build(stream: bool = False) -> bool:
@@ -118,7 +113,7 @@ def harness_needs_build(stream: bool = False) -> bool:
 
 
 def build_harness(force: bool = False, stream: bool = False) -> str:
-    """Compile the kernel test harness (stream=True: the streaming harness) next to libbv2.so with the product flags (no -DBV2_TUNING)."""
+    """Compile the kernel test harness (stream=True: the streaming harness) next to libbv2.so with the product flags."""
     src, path = (STREAM_HARNESS_SOURCE, STREAM_HARNESS_PATH) if stream else (HARNESS_SOURCE, HARNESS_PATH)
     with _lock:
         if not force and not harness_needs_build(stream):
@@ -136,11 +131,10 @@ def load():
     global _lib
     if _lib is not None:
         return _lib
-    path = os.environ.get("BV2_LIB") or LIB_PATH  # BV2_LIB: development A/B runs against libbv2_tuning.so
-    if not os.path.isfile(path):
-        raise RuntimeError(f"{path} not built; run `python -c 'import __graft_entry__ as g; g.build()'`. "
+    if not os.path.isfile(LIB_PATH):
+        raise RuntimeError(f"{LIB_PATH} not built; run `python -c 'import __graft_entry__ as g; g.build()'`. "
                            "There is no CPU/PyTorch fallback for the engine.")
-    lib = C.CDLL(path)
+    lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SYMBOLS.items():
         fn = getattr(lib, name)
         fn.restype = res

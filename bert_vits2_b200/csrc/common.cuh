@@ -66,17 +66,12 @@ static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 // kernel launched this way executes `griddepcontrol.wait` (pdl_wait()) before touching data produced upstream.
 template <typename... KArgs, typename... Args>
 inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
-#ifdef BV2_TUNING
-    static const int pdl_env = getenv("BV2_PDL") ? atoi(getenv("BV2_PDL")) : 1;  // development builds only
-#else
-    const int pdl_env = 1;
-#endif
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl_env ? 1 : 0;
+    cfg.attrs = attr; cfg.numAttrs = 1;
     BV2_CUDA(cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...));
 }
 // Same, with a thread-block cluster of cluster_x CTAs along x (grid.x must be a multiple of cluster_x)

@@ -268,7 +268,7 @@ struct bv2_engine {
             L.relv = upload(W(a + ".emb_rel_v").data);
             L.n1 = ln_from(name + ".norm_layers_1." + std::to_string(i));
             L.f1 = conv_from(name + ".ffn_layers." + std::to_string(i) + ".conv_1", false, tc_mode, 128, 64);
-            L.f2 = conv_from(name + ".ffn_layers." + std::to_string(i) + ".conv_2", false, tc_mode, tune_env("BV2_F2_NT", 32), 64);  // (BV2_F2_NT=192 in a tuning build: one N tile with the LayerNorm in the tail; measured 10 us per layer slower, r02d)
+            L.f2 = conv_from(name + ".ffn_layers." + std::to_string(i) + ".conv_2", false, tc_mode, 32, 64);  // (one 192-column N tile with the LayerNorm in the tail measured 10 us per layer slower)
             L.n2 = ln_from(name + ".norm_layers_2." + std::to_string(i));
             e.layers.push_back(L);
         }
@@ -340,7 +340,6 @@ struct bv2_engine {
     // token-rate FP32 conv through the cluster split-K kernel (kernels_tok.cuh); false -> caller uses the generic path
     bool tok_conv(const ConvW& cw, const Act& x, const Act& y, cudaStream_t s, const ConvArgs& e, const LnW* ln = nullptr, const float* ln_res = nullptr,
                   int mask_pre = 0, int cout_off = 0) {
-        if (!tune_env("BV2_TOK_GEMM", 1)) return false;
         TokGemmArgs a{};
         a.x = x.p; a.Cin_total = x.C; a.cin_off = 0; a.Cin = cw.Cin;
         a.w = cw.w; a.Cout_w = cw.Cout_w; a.bias = cw.b; a.bias_b = e.bias_b; a.bias_b_stride = e.bias_b_stride;
@@ -559,13 +558,13 @@ void bv2_engine::build_weights() {
     const int half = I / 2, n = c.n_flows;
     flows.resize(n);
     // generator_precision: 0 = fp32 SIMT everywhere; 1 = TF32 wgmma (flow + Generator); 2 = FP16-operand wgmma Generator
-    // (same 11-bit significand as TF32, fp32 accumulate, fp32 activations in HBM) + TF32 flow
+    // (same 11-bit significand as TF32, fp32 accumulate, 16-bit activations in HBM: k_g2_conv, tc_gen.cuh) + TF32 flow
     // 3 = FP16 operands in the flow too, with the fused attention kernel (tc_attn.cuh)
     const int tc = c.generator_precision == 3 ? 2 : (c.generator_precision ? 1 : 0);
     const int gtc = c.generator_precision >= 2 ? 2 : tc;
     flow_tc = tc;
     if (tc == 2) tc_flow_attn_init_device();
-    use_g2 = (gtc == 2 && tune_env("BV2_G2", 1)) ? 1 : 0;
+    use_g2 = gtc == 2 ? 1 : 0;
     if (use_g2) g2_init_device();
     for (int i = 0; i < n; i++) {
         CouplingW& fl = flows[i];
@@ -651,7 +650,7 @@ void bv2_engine::build_weights() {
                 for (int j = 0; j < u.K; j++) p[((size_t)ci * u.K + j) * u.Cout + co] = w[((size_t)ci * u.Cout + co) * u.K + j];
         u.w = upload(p); u.b = upload(W("dec.ups." + std::to_string(i) + ".bias").data);
         if (use_g2) u.tc = tc_pack_upsample(*this_uploader(), w, u.Cin, u.Cout, u.K, u.u, g2_kc(u.Cin), 1, packing(), 128);
-        else if (gtc) u.tc = tc_pack_upsample(*this_uploader(), w, u.Cin, u.Cout, u.K, u.u, 32, gtc == 2, packing());
+        else if (gtc) u.tc = tc_pack_upsample(*this_uploader(), w, u.Cin, u.Cout, u.K, u.u, 32, 0, packing());
         ups.push_back(u);
         ch /= 2;
         for (int j = 0; j < c.n_resblock_kernels; j++) {
@@ -660,7 +659,7 @@ void bv2_engine::build_weights() {
             for (int d = 0; d < c.n_dilations; d++) {
                 rb.dil.push_back(c.resblock_dilation_sizes[j][d]);
                 const int kc = use_g2 ? g2_kc(ch) : 32;  // persistent kernels hide latency with deep rings: fewer, larger chunks
-                const int nt0 = use_g2 ? g2_nt(ch) : (ch >= 256 ? tune_env("BV2_S0_NT", 0) : 0);  // tuning knob (stage 0 N tile)
+                const int nt0 = use_g2 ? g2_nt(ch) : 0;
                 rb.c1.push_back(conv_from(r + ".convs1." + std::to_string(d), true, gtc, nt0, kc));
                 rb.c2.push_back(conv_from(r + ".convs2." + std::to_string(d), true, gtc, nt0, kc));
             }
@@ -711,18 +710,10 @@ void bv2_engine::run_encoder(const EncoderW& E, Act x, const int* lens, const fl
                 ConvArgs a1; a1.in_mask = 1; a1.act = 1; a1.out_mask = 1; a1.lens = lens;
                 tc_out_f16 = 1;
                 conv(L.f1, x, f16, s, a1, 0, 0, true);
-                if (L.f2.tc.nt == H) {
-                    // x = norm_2(x + ffn(x)): conv_2 on one full-width N tile, LayerNorm in the tail, residual tile staged by TMA
-                    // (rows t >= len skip the reference's y * x_mask; they only ever feed masked positions and are zeroed by the last layer)
-                    ConvArgs a2; a2.lens = lens; a2.res = x.p; a2.res_mode = 1; a2.res_C_total = H; a2.out_mask = i == nl - 1 ? 1 : 0;
-                    tc_in_f16 = 1; tc_ln = &L.n2;
-                    conv(L.f2, f16, x, s, a2, 0, 0, true);
-                } else {
-                    ConvArgs a2; a2.out_mask = 1; a2.lens = lens;
-                    tc_in_f16 = 1;
-                    conv(L.f2, f16, y, s, a2, 0, 0, true);
-                    layernorm(L.n2, x, y.p, x, s, 0, nullptr, lens, i == nl - 1 ? 1 : 0);
-                }
+                ConvArgs a2; a2.out_mask = 1; a2.lens = lens;
+                tc_in_f16 = 1;
+                conv(L.f2, f16, y, s, a2, 0, 0, true);
+                layernorm(L.n2, x, y.p, x, s, 0, nullptr, lens, i == nl - 1 ? 1 : 0);
             }
             continue;
         }
@@ -788,7 +779,7 @@ void bv2_engine::run_dds(const DdsW& D, Act x, const int* lens, cudaStream_t s) 
     const int B = x.B, T = x.T, C = x.C;
     const size_t mark = ws.used();
     const int nl0 = (int)D.c1.size();
-    if (C == 192 && nl0 >= 2 && tune_env("BV2_DDS_FUSED", 1)) {
+    if (C == 192 && nl0 >= 2) {
         // one launch per layer (kernels_tok.cuh); the layer reads a +-dilation halo, so it ping-pongs between buffers and the last
         // layer lands in x again
         Act tmp[2] = {ws.act(B, C, T), ws.act(B, C, T)};
@@ -829,7 +820,7 @@ void bv2_engine::run_text_encoder(int B, int T, const int64_t* x, const int64_t*
     const int H = cfg.hidden_channels, D = cfg.bert_dim;
     Act proj = ws.act(B, H, T);
     bool done = false;
-    if (tune_env("BV2_TOK_GEMM", 1) && H == 192) {
+    if (H == 192) {
         // BERT ingest (SURVEY.md section 8f.3): the three [B,1024,T] feature tensors are read in the layout get_text hands them over,
         // one K = 3072 contraction on the cluster split-K kernel (no staging transposes, no intermediate tensor)
         TokGemmArgs a{};

@@ -36,7 +36,6 @@ struct AttnParams {
     int B, T, H, heads, window;
     int ks;             // key split: a cluster of ks CTAs shares one 128-query tile, CTA r takes key tiles r, r + ks, ... (1 = no cluster)
     uint32_t v_lbo, v_sbo;  // MN-major descriptor strides of the V operand
-    long long* prof;    // probes only: per-CTA globaltimer stamps [ctas][10]; nullptr in the engine
 };
 
 namespace tc {
@@ -144,10 +143,6 @@ __global__ void __launch_bounds__(288, 1) k_flow_attn(AttnParams p) {
     const int q0 = ((int)blockIdx.x / KS) * 128, h = blockIdx.y, b = blockIdx.z;
     const int H8 = p.H / 8;
     const int w = p.window, nrel = 2 * w + 1;
-    auto gtimer = [] { long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; };
-    long long* prof = p.prof ? p.prof + ((size_t)(blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 10 : nullptr;
-    const bool stamp = prof && threadIdx.x == 0;
-    if (stamp) prof[0] = gtimer();
 
     if (threadIdx.x == 0) {
         mbar_init(BAR(B_QFULL), 1);
@@ -162,7 +157,6 @@ __global__ void __launch_bounds__(288, 1) k_flow_attn(AttnParams p) {
     __syncthreads();
     asm volatile("griddepcontrol.wait;" ::: "memory");
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    if (stamp) prof[1] = gtimer();
 
     const int len = min(p.lens ? p.lens[b] : p.T, p.T);
     const int NT_all = q0 < len ? (len + KT - 1) / KT : 0;  // key tiles that hold at least one valid key (same for the whole cluster)
@@ -238,7 +232,6 @@ __global__ void __launch_bounds__(288, 1) k_flow_attn(AttnParams p) {
                 for (int r = 0; r < NREL; r++) { sQrel[r * 128 + m] = qrel[r]; sPrel[r * 128 + m] = 0.f; }
             }
             asm volatile("bar.sync 1, 256;" ::: "memory");  // both consumer warpgroups: the qrel / prel tables are complete
-            if (stamp) prof[2] = gtimer();
             const uint64_t qd = make_desc(smem_u32(sQ), 128u * 16u, 128u) + (uint64_t)(64 * wg);  // 64 rows further = 8 core-matrix groups
             // S (64 rows x KT keys of this warpgroup) = Q . K_tile^T, then the K stage goes back to the producer
             auto scores = [&](int s, float* c) {
@@ -274,7 +267,6 @@ __global__ void __launch_bounds__(288, 1) k_flow_attn(AttnParams p) {
                 M[hr] = fmaxf(M[hr], __shfl_xor_sync(0xffffffffu, M[hr], 1));
                 M[hr] = fmaxf(M[hr], __shfl_xor_sync(0xffffffffu, M[hr], 2));
             }
-            if (stamp) prof[3] = gtimer();
             // ---- pass B: p = exp(s - M) in registers -> P.V; row sums; relative-value weights
             const float M2[2] = {M[0] * LOG2E, M[1] * LOG2E};
             for (int j = 0; j < NT; j++) {
@@ -315,7 +307,6 @@ __global__ void __launch_bounds__(288, 1) k_flow_attn(AttnParams p) {
                 L[hr] += __shfl_xor_sync(0xffffffffu, L[hr], 1);
                 L[hr] += __shfl_xor_sync(0xffffffffu, L[hr], 2);
             }
-            if (stamp) prof[4] = gtimer();
         }
         // ---- park this CTA's partial rows in its own shared memory (the K/V stages, free once both warpgroups are done):
         //      [27 float4][128 rows]: slots 0..23 unnormalised P.V (96 channels), 24 = (m, l, prel0, prel1), 25 = prel2..5, 26 = prel6..8
@@ -340,13 +331,10 @@ __global__ void __launch_bounds__(288, 1) k_flow_attn(AttnParams p) {
                 part[(size_t)26 * 128 + row] = make_float4(pr[6], pr[7], pr[8], 0.f);
             }
         }
-        if (stamp) prof[5] = gtimer();
     }
     if (NT_all > 0) {
         // ---- merge the key splits (every thread of every CTA of the cluster takes part in both barriers)
-        if (stamp) prof[6] = gtimer();
         asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-        if (stamp) prof[7] = gtimer();
         // CTA rk merges rows [rk * 128/KS, (rk + 1) * 128/KS); KS threads share a row (96/KS channels each), consecutive threads take
         // consecutive rows (coalesced distributed-shared-memory reads)
         if (threadIdx.x < 128) {
@@ -354,10 +342,8 @@ __global__ void __launch_bounds__(288, 1) k_flow_attn(AttnParams p) {
             else if (KS == 2) attn_merge_rows<2, DK>(smem_u32(sK), sEv, rk, threadIdx.x, q0, len, p.T, nrel, obase);
             else attn_merge_rows<1, DK>(smem_u32(sK), sEv, rk, threadIdx.x, q0, len, p.T, nrel, obase);
         }
-        if (stamp) prof[8] = gtimer();
         asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");  // peers are done reading this CTA's rows
     }
-    if (stamp) prof[9] = gtimer();
 }
 
 inline size_t tc_flow_attn_smem(int DK, int KT) { return (size_t)DK * 128 * 2 + 4 * (size_t)DK * KT * 2 + 2 * 9 * (size_t)DK * 4 + 2 * 9 * 128 * 4 + 9 * 8 + 16; }
@@ -368,13 +354,13 @@ inline void tc_flow_attn_init_device() {
 
 // qkv16: 16-bit c8 tensor with C = 3H channels (Act.p reinterpreted); att16: 16-bit c8 tensor with C = H channels.
 inline void tc_flow_attn(const Act& qkv16, const Act& att16, const float* rel_k, const float* rel_v, const int* lens, int heads, int window,
-                         cudaStream_t st, int num_sms, int ks_override = 0, long long* prof = nullptr) {
+                         cudaStream_t st, int num_sms, int ks_override = 0) {
     const int H = att16.C, dk = H / heads, KT = 128;
     BV2_CHECK(qkv16.C == 3 * H && dk == 96 && H % 8 == 0 && window <= 4 && qkv16.T == att16.T && qkv16.B == att16.B, "tc_flow_attn shapes (head dim 96, window <= 4)");
     AttnParams p{};
     p.qkv = reinterpret_cast<const uint4*>(qkv16.p); p.att = reinterpret_cast<uint4*>(att16.p);
     p.rel_k = rel_k; p.rel_v = rel_v; p.lens = lens;
-    p.B = qkv16.B; p.T = qkv16.T; p.H = H; p.heads = heads; p.window = window; p.prof = prof;
+    p.B = qkv16.B; p.T = qkv16.T; p.H = H; p.heads = heads; p.window = window;
     p.v_lbo = 128u;                 // MN-major V: stride between 8-key core-matrix blocks (K direction)
     p.v_sbo = (uint32_t)KT * 16u;   // ... and between 8-channel blocks (N direction)
     // key split: as many CTAs per query tile as keep the grid within one wave of the SMs and leave each CTA at least one key tile

@@ -60,7 +60,6 @@ struct TcEpi {
     int out_f16 = 0;     // store y as a 16-bit c8 tensor
     int gate = 0;        // WN gate fused into the tail (reference commons.py:98-105): columns (2c, 2c+1) hold the tanh / sigmoid pre-activations of
                          // channel c (weights interleaved at load time); y gets tanh(a) * sigmoid(b) as a 16-bit c8 tensor with Cout/2 channels
-    long long* prof = nullptr;  // probes: per-CTA phase timestamps (k_tc_conv1d)
     const float* ln_gamma = nullptr; const float* ln_beta = nullptr;  // LayerNorm over the Cout channels of each time step fused into the
                                                                       // tail (one N tile = all channels; combine with res for norm(x + conv))
 };
@@ -84,17 +83,6 @@ inline float f16_round_host(float x) {
     return __half2float(h);
 }
 
-// Tuning knobs are compiled out of the product build (-DBV2_TUNING enables the BV2_* environment variables for probes).
-inline int tune_env(const char* name, int dflt) {
-#ifdef BV2_TUNING
-    const char* v = getenv(name);
-    return v ? atoi(v) : dflt;
-#else
-    (void)name;
-    return dflt;
-#endif
-}
-
 // w: [Cout][Cin][K] fp32 (weight-norm already folded)
 // nt = N tile (0: largest divisor of Cout that is a multiple of 16 and <= 128: a 128-column fp32 accumulator image is 66 KB of shared memory)
 // kc = K chunk (channels per pipeline stage)
@@ -104,7 +92,6 @@ inline TcConvW tc_pack_weights(std::function<float*(const std::vector<float>&)>&
                                int f16 = 0, int kc = 0, bool fill = true) {
     TcConvW t; t.Cin = Cin; t.Cout = Cout; t.K = K; t.f16 = f16;
     if (!nt) { nt = std::min(Cout, 128); while (Cout % nt || nt % 16) nt -= 16; }
-    kc = tune_env("BV2_TC_KC", kc);
     if (!kc) kc = 32;
     t.KC = Cin >= kc ? kc : Cin;
     const int G = f16 ? 8 : 4;
@@ -184,7 +171,6 @@ struct TcParams {
     long long w_zstride;        // packed-weight offset per z (floats)
     int w_mode;                 // 1: B operand rows come from a c4 activation tensor (K == 1): w = tensor base
     int w_ld, w_rows, w_c_total, w_c_off, w_c_zstride;
-    long long* prof;            // probes only: per-CTA globaltimer stamps [ctas][8] (k_tc_conv1d); nullptr in the engine
 };
 
 // Device-side error flags: a barrier timeout raises both and lets the kernel run to completion instead of trapping the context
@@ -652,9 +638,6 @@ __global__ void __launch_bounds__(384, 1) k_tc_conv1d(TcParams p) {
     // that touch only static data do not wait for it: the weight producer fills its ring and, when the accumulator init is bias-only,
     // the epilogue warps pre-load the accumulators while the upstream kernel is still running.  Everybody else waits, then releases
     // the dependents (releasing them before the wait would let the whole rest of the stream become resident at once).
-    auto gtimer = [] { long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; };
-    long long* prof = p.prof ? p.prof + ((size_t)(blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 8 : nullptr;
-    if (prof && threadIdx.x == 0) prof[0] = gtimer();
     // LayerNorm tail with a TMA-staged residual (p.res_soff): the residual tile is copied into shared memory by the activation producer
     // right after the PDL wait and added by the tail, so the accumulator init is bias-only (static data, runs ahead of the wait) and the
     // MMAs never wait for residual loads (pre-loading the residual into the accumulator means dependent rounds of float4 loads per
@@ -666,7 +649,6 @@ __global__ void __launch_bounds__(384, 1) k_tc_conv1d(TcParams p) {
         asm volatile("griddepcontrol.wait;" ::: "memory");
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     }
-    if (prof && threadIdx.x == 0) prof[1] = gtimer();
 
     const int R = p.R;
     const int G = F16 ? 8 : 4;                                  // channels per 16-byte operand group
@@ -756,7 +738,6 @@ __global__ void __launch_bounds__(384, 1) k_tc_conv1d(TcParams p) {
             uint64_t a_cur = a_desc_base, b_cur = b_desc_base;
             for (int c = 0; c < p.nchunks; c++) {
                 mbar_wait_u(bar_ar + 8u * sa, aph);
-                if (prof && c == 0 && lane == 0) prof[2] = gtimer();
                 uint64_t a_tap = a_cur;
                 for (int j = 0; j < p.K; j++, a_tap += (uint64_t)(uint32_t)p.dil) {
                     mbar_wait_u(bar_wf + 8u * sw, wph);
@@ -771,7 +752,6 @@ __global__ void __launch_bounds__(384, 1) k_tc_conv1d(TcParams p) {
                 if (++sa == nas_u) { sa = 0; aph ^= 1u; a_cur = a_desc_base; }
             }
             wg_commit(BAR(B_ACC));
-            if (prof && lane == 0) prof[3] = gtimer();
         }
     } else if (warp == 1 || warp == 7) {  // idle (the MMA warpgroup starts at a warpgroup boundary)
     } else {
@@ -781,7 +761,6 @@ __global__ void __launch_bounds__(384, 1) k_tc_conv1d(TcParams p) {
         for (int mt = 0; mt < MT; mt++)
             acc_init_tile<4, GEN>(p, acc0 + ((uint32_t)(q * 32) << 16) + (uint32_t)(mt * nt), b, t0 + mt * 128 + q * 32 + lane, n0, nt, yb, cout_off, res_smem);
         mbar_arrive(BAR(B_INIT));
-        if (prof && tid2 == 0) prof[4] = gtimer();
         if (bias_only) {  // the init above touched static data only; everything below reads / overwrites tensors of the upstream kernel
             asm volatile("griddepcontrol.wait;" ::: "memory");
             asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -793,7 +772,6 @@ __global__ void __launch_bounds__(384, 1) k_tc_conv1d(TcParams p) {
         for (int c = 0; c < p.nchunks; c++) {
             const int sa = c % NAS;
             mbar_wait(BAR(B_AFULL + sa), (c / NAS) & 1);
-            if (prof && tid2 == 0 && c == 0) prof[7] = gtimer();
             uint8_t* st = sA + (size_t)sa * p.a_stage_bytes;
             if (F16) {
                 if (!p.in_f16) xform16_stage(reinterpret_cast<const float4*>(st), reinterpret_cast<uint4*>(st + p.a_op_off), p.KC / 8, R, r_lo, r_mask_hi, slope, tid2);
@@ -815,7 +793,6 @@ __global__ void __launch_bounds__(384, 1) k_tc_conv1d(TcParams p) {
         }
         // ===== tail
         mbar_wait(BAR(B_ACC), 0);
-        if (prof && tid2 == 0) prof[5] = gtimer();
         if (GEN && p.ln_gamma) {
             const float4* rs = nullptr;
             if (res_smem) { mbar_wait(BAR(B_RES), 0); rs = reinterpret_cast<const float4*>(smem + p.res_soff) + (q * 32 + lane); }
@@ -824,7 +801,6 @@ __global__ void __launch_bounds__(384, 1) k_tc_conv1d(TcParams p) {
             for (int mt = 0; mt < MT; mt++)
                 acc_tail_tile<4, GEN>(p, acc0 + ((uint32_t)(q * 32) << 16) + (uint32_t)(mt * nt), b, t0 + mt * 128 + q * 32 + lane, n0, nt, len, yb, cout_off);
         }
-        if (prof && tid2 == 0) prof[6] = gtimer();
     }
     __syncthreads();
 }
@@ -1130,7 +1106,7 @@ __global__ void __launch_bounds__(512, 1) k_tc_conv1d_pstream(TcParams p, int mt
 // host side
 // ------------------------------------------------------------------------------------------------------------
 // The > 48 KB dynamic shared memory opt-in is a per-device (per-context) function attribute: call once per device before
-// the first launch there (bv2_engine::finalize does; probes call it themselves).
+// the first launch there (bv2_engine::finalize does; the kernel test harness calls it itself).
 inline void tc_clear_error() {
     const int z = 0;
     BV2_CUDA(cudaMemcpyToSymbol(g_tc_err_dev, &z, sizeof(z)));
@@ -1198,7 +1174,7 @@ inline TcConvPlan tc_conv_plan(const TcConvW& w, const float* bias, const Act& x
     p.in_slope = e.in_slope; p.out_scale = e.out_scale; p.accumulate = e.accumulate; p.relu = e.relu; p.res_mode = e.res ? (e.res_mode ? e.res_mode : 1) : 0;
     p.in_mask = e.in_mask; p.out_mask = e.out_mask; p.ups_u = w.ups_u; p.ups_cout = w.ups_cout;
     p.out_tf32 = e.out_tf32; p.skip_xform = e.skip_xform; p.in_f16 = e.in_f16; p.out_f16 = e.out_f16;
-    p.ln_gamma = e.ln_gamma; p.ln_beta = e.ln_beta; p.gate = e.gate; p.prof = e.prof;
+    p.ln_gamma = e.ln_gamma; p.ln_beta = e.ln_beta; p.gate = e.gate;
     if (e.gate) BV2_CHECK(F16 && !w.ups_u && !e.res && !e.accumulate && !e.relu && !e.out_f16 && !e.ln_gamma && e.cout_off % 8 == 0 && y.C % 8 == 0 && 2 * y.C >= w.Cout, "gate epilogue");
     if (e.ln_gamma) BV2_CHECK(e.ln_beta && ntiles == 1 && nt % 32 == 0 && !w.ups_u && !e.out_f16 && !e.out_tf32 && !e.relu && e.out_scale == 1.f && e.res_mode != 2 && e.cout_off % 4 == 0, "LayerNorm tail needs one N tile holding every channel");
     if (e.skip_xform) BV2_CHECK(!F16 && w.K == 1 && e.in_slope == 1.f && !e.in_mask, "skip_xform needs a TF32 plain 1x1 conv input");
@@ -1220,7 +1196,7 @@ inline TcConvPlan tc_conv_plan(const TcConvW& w, const float* bias, const Act& x
 
     // ---- narrow layer with many tiles: persistent CTAs, resident weights, double-buffered accumulator image
     const size_t w_all = (size_t)p.K * p.KC * nt * esz;
-    if (tune_env("BV2_TC_PERSIST", 1) && !e.skip_xform && !e.in_f16 && !e.out_f16 && !e.ln_gamma && !e.gate && p.nchunks == 1 && ntiles == 1 && w_all <= 64 * 1024 && nctas >= 2 * num_sms) {
+    if (!e.skip_xform && !e.in_f16 && !e.out_f16 && !e.ln_gamma && !e.gate && p.nchunks == 1 && ntiles == 1 && w_all <= 64 * 1024 && nctas >= 2 * num_sms) {
         p.nas = 3;
         const size_t wb = (w_all + 127) & ~(size_t)127;
         p.acc_cols = (uint32_t)(2 * nt);
@@ -1235,7 +1211,7 @@ inline TcConvPlan tc_conv_plan(const TcConvW& w, const float* bias, const Act& x
     }
     // ---- wide layer with at least one tile per SM: persistent CTAs, continuously streamed weights, double-buffered accumulator image
     // (only when two activation and two weight stages fit next to the double-buffered accumulator image; otherwise one tile per CTA)
-    if (tune_env("BV2_TC_PSTREAM", 1) && !e.skip_xform && !e.in_f16 && !e.ln_gamma && nctas >= num_sms && nt >= 64 &&
+    if (!e.skip_xform && !e.in_f16 && !e.ln_gamma && nctas >= num_sms && nt >= 64 &&
         tc::acc_img_bytes((uint32_t)(2 * nt)) + 2ull * p.a_stage_bytes + 2ull * p.w_stage_bytes + 2048 <= 220 * 1024) {
         // 128-row tiles: the double-buffered accumulator image (2 x nt columns) already takes up to 132 KB of shared memory
         const int MT = 1;
@@ -1259,13 +1235,13 @@ inline TcConvPlan tc_conv_plan(const TcConvW& w, const float* bias, const Act& x
     }
     // ---- one tile per CTA.  Shared memory per CTA is capped (~48 KB) when there are more CTAs than SMs so that several
     // CTAs co-reside: one CTA's accumulator init / tail overlaps the other's MMA main loop
-    uint32_t budget = (nctas > num_sms && nt <= 128) ? (uint32_t)tune_env("BV2_TC_SMEM_KB", 48) * 1024 : 200 * 1024;
+    uint32_t budget = (nctas > num_sms && nt <= 128) ? 48 * 1024 : 200 * 1024;
     if (nt > 128 && 2 * nctas > num_sms && 2ull * p.a_stage_bytes + 2ull * p.w_stage_bytes + 2048 <= 112 * 1024)
         budget = 112 * 1024;  // wide layer launched on three streams at once (MRF resblock chains): let two CTAs share an SM
     // LayerNorm tail with a residual, at most one CTA per SM (small batches: the launch is a latency chain, not a throughput problem):
     // the residual tile is staged in shared memory by TMA (nt/4 channel groups x 128 rows x 16 B) instead of being pre-loaded into the
     // accumulator; the rings shrink to make room (the weight ring never needs more stages than the conv has)
-    const bool res_smem = e.ln_gamma && p.res_mode == 1 && !p.accumulate && nctas <= num_sms && p.res_c_off % 4 == 0 && tune_env("BV2_LN_RES_SMEM", 1) &&
+    const bool res_smem = e.ln_gamma && p.res_mode == 1 && !p.accumulate && nctas <= num_sms && p.res_c_off % 4 == 0 &&
                           tc::acc_img_bytes((uint32_t)nt) + (size_t)nt * 512u + 2ull * p.a_stage_bytes + 2ull * p.w_stage_bytes + 2048 <= 224 * 1024;
     const uint32_t res_bytes = res_smem ? (uint32_t)nt * 512u : 0u;
     const uint32_t img = tc::acc_img_bytes((uint32_t)nt);
@@ -1275,7 +1251,7 @@ inline TcConvPlan tc_conv_plan(const TcConvW& w, const float* bias, const Act& x
     while (nas > 2 && (size_t)nas * p.a_stage_bytes + 4 * (size_t)p.w_stage_bytes + 1024 > budget) nas--;
     p.nas = nas;
     int nws = ((int)budget - nas * (int)p.a_stage_bytes - 1024) / (int)p.w_stage_bytes;
-    p.nws = std::max(2, std::min(nws, tune_env("BV2_TC_NWS_MAX", 8)));
+    p.nws = std::max(2, std::min(nws, 8));
     p.nws = std::max(2, std::min(p.nws, p.nchunks * p.K));
     p.acc_cols = (uint32_t)nt;
     size_t smem = img + (size_t)p.nas * p.a_stage_bytes + (size_t)p.nws * p.w_stage_bytes + (size_t)(3 * p.nas + 2 * p.nws + 3) * 8 + 16;

@@ -47,15 +47,9 @@ struct G2Params {
     uint32_t a_stage_bytes, w_stage_bytes, acc_cols;  // acc_cols: columns of the accumulator image
     int residual, accumulate, ups_u, ups_cout;
     float out_scale;
-    int dbg_skip_wcommit;  // probes only: no weight-stage commits (valid only when every weight stage fits the ring)
-    int dbg_flags;         // probes only (timing studies, wrong results): 1 = no tap shift (aligned A operand), 2 = no wgmma fence after the stage waits,
-                           // 4 = no TMA traffic after the first ring fill (stale operands re-used: isolates shared-memory contention), 8 = epilogue warps
-                           // park in nanosleep polling instead of the hinted try_wait, 16 = no halo zeroing of the output
-    long long* prof;  // probes only: per-CTA timestamps [grid][16] (globaltimer ns / clock64 sums); nullptr in the engine
 };
 
 namespace tc {
-__device__ __forceinline__ long long gtime() { long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 __device__ __forceinline__ void unpack8(const uint4& u, float* f) {
     const __half2* h = reinterpret_cast<const __half2*>(&u);
 #pragma unroll
@@ -77,37 +71,29 @@ __device__ __forceinline__ void g2_issue_stage(uint32_t d0, uint32_t a_lo0, uint
 struct G2Issue {
     uint32_t bar_af, bar_ae, bar_wf, bar_we, bar_acc;      // first barrier of each group
     uint32_t a_lo_base, w_lo_base, a_stage16, w_stage16;   // descriptor low words of ring slot 0, slot strides (16-byte units)
-    uint32_t a_kstep, b_kstep, nt, tapstep, tm;
+    uint32_t a_kstep, b_kstep, nt, dil, tm;
     uint32_t nas, nws;
-    int NG, NCH, K, streamed, wcommit, nostale;
+    int NG, NCH, K, streamed;
     uint64_t hi;
 };
 
 // The issuer's loop nest for one (NK, MG) instantiation.  Ring slots, parities, barrier addresses and descriptor words are carried
 // incrementally (adds and compares only: no runtime integer division in front of every stage's MMAs).
 template <int NK, int MG>
-__device__ __forceinline__ void g2_issuer(const G2Issue& q, long long* prof, int lane) {
+__device__ __forceinline__ void g2_issuer(const G2Issue& q) {
     using namespace tc;
     uint32_t sa = 0, aph = 0, a_cur = q.a_lo_base;   // activation ring slot, parity, descriptor low word of the slot
     uint32_t sw = 0, wph = 0, w_cur = q.w_lo_base;   // weight ring (streamed) / tap cursor (resident)
     uint32_t dg = q.tm;
-    int s = 0, wi = 0;
-    long long waitA = 0, waitW = 0;
     for (int g = 0; g < q.NG; g++, dg += (uint32_t)MG * q.nt) {
         if (!q.streamed) w_cur = q.w_lo_base;
-        for (int c = 0; c < q.NCH; c++, s++) {
-            long long c0 = prof ? clock64() : 0;
-            if (q.nostale || s < (int)q.nas) mbar_wait_u(q.bar_af + 8u * sa, aph);
-            if (prof) { waitA += clock64() - c0; if (s == 0 && lane == 0) { prof[3] = gtime(); prof[10] = clock64(); } }
+        for (int c = 0; c < q.NCH; c++) {
+            mbar_wait_u(q.bar_af + 8u * sa, aph);
             uint32_t a_tap = a_cur;
-            for (int j = 0; j < q.K; j++, wi++, a_tap += q.tapstep) {
-                if (q.streamed) {
-                    c0 = prof ? clock64() : 0;
-                    if (q.nostale || wi < (int)q.nws) mbar_wait_u(q.bar_wf + 8u * sw, wph);
-                    if (prof) waitW += clock64() - c0;
-                }
+            for (int j = 0; j < q.K; j++, a_tap += q.dil) {
+                if (q.streamed) mbar_wait_u(q.bar_wf + 8u * sw, wph);
                 g2_issue_stage<NK, MG>(dg, a_tap, w_cur, q.a_kstep, q.b_kstep, q.hi, q.nt);
-                if (q.wcommit) wg_commit(q.bar_we + 8u * sw);
+                if (q.streamed) wg_commit(q.bar_we + 8u * sw);
                 w_cur += q.w_stage16;
                 if (q.streamed && ++sw == q.nws) { sw = 0; wph ^= 1u; w_cur = q.w_lo_base; }
             }
@@ -117,18 +103,17 @@ __device__ __forceinline__ void g2_issuer(const G2Issue& q, long long* prof, int
         }
         wg_commit(q.bar_acc + 8u * (uint32_t)g);
     }
-    if (prof && lane == 0) { prof[4] = gtime(); prof[8] = waitA; prof[9] = waitW; prof[11] = clock64(); prof[12] = (long long)q.NG * q.NCH * q.K * MG * NK; }
 }
 // MG dispatch as a binary tree of two-way branches (a switch would become a jump table: BRX on a vector register makes ptxas treat
 // the code after it as divergent and takes the descriptors out of the uniform datapath)
 template <int NK>
-__device__ __forceinline__ void g2_issuer_mg(const G2Issue& q, int MG, long long* prof, int lane) {
+__device__ __forceinline__ void g2_issuer_mg(const G2Issue& q, int MG) {
     if (MG <= 4) {
-        if (MG <= 2) { if (MG == 1) g2_issuer<NK, 1>(q, prof, lane); else g2_issuer<NK, 2>(q, prof, lane); }
-        else { if (MG == 3) g2_issuer<NK, 3>(q, prof, lane); else g2_issuer<NK, 4>(q, prof, lane); }
+        if (MG <= 2) { if (MG == 1) g2_issuer<NK, 1>(q); else g2_issuer<NK, 2>(q); }
+        else { if (MG == 3) g2_issuer<NK, 3>(q); else g2_issuer<NK, 4>(q); }
     } else {
-        if (MG <= 6) { if (MG == 5) g2_issuer<NK, 5>(q, prof, lane); else g2_issuer<NK, 6>(q, prof, lane); }
-        else { if (MG == 7) g2_issuer<NK, 7>(q, prof, lane); else g2_issuer<NK, 8>(q, prof, lane); }
+        if (MG <= 6) { if (MG == 5) g2_issuer<NK, 5>(q); else g2_issuer<NK, 6>(q); }
+        else { if (MG == 7) g2_issuer<NK, 7>(q); else g2_issuer<NK, 8>(q); }
     }
 }
 
@@ -139,8 +124,6 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;  // shfl: warp-uniform for the compiler
     const int NAS = p.nas, NWS = p.nws, NG = p.NG, MG = p.MG, NCH = p.nchunks, nt = p.nt, R = p.R;
     const int t0 = p.t_begin + blockIdx.x * NG * MG * 128, ntile = blockIdx.y, n0 = ntile * nt, b = blockIdx.z;
-    long long* prof = p.prof ? p.prof + ((size_t)(blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 16 : nullptr;
-    if (prof && threadIdx.x == 0) prof[0] = gtime();
     uint8_t* sA = smem;
     uint8_t* sW = smem + (size_t)NAS * p.a_stage_bytes;
     const int nwst = p.resident ? NCH * p.K : NWS;  // weight stages held in shared memory
@@ -163,16 +146,13 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
 
     if (warp == 0) {
         // ===== activation producer (reads the upstream kernel's output: PDL wait first)
-        if (prof && lane == 0) prof[1] = gtime();
         asm volatile("griddepcontrol.wait;" ::: "memory");
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-        if (prof && lane == 0) prof[2] = gtime();
         const int steps = NG * NCH;
         for (int s = 0; s < steps; s++) {
             const int g = s / NCH, c = s - g * NCH, sa = s % NAS;
             const int row0 = t0 + g * MG * 128 - p.pad;
             const int nrows = max(0, min(R, p.T + G2_PADR - row0));  // never read past the tensor's halo; rows beyond (and rows past a window's end) feed discarded outputs only
-            if ((p.dbg_flags & 4) && s >= NAS) continue;
             if (lane == 0) {
                 mbar_wait(BAR(B_AEMPTY + sa), ((s / NAS) & 1) ^ 1);
                 mbar_expect_tx(BAR(B_AFULL + sa), (uint32_t)nrows * 16u * (uint32_t)ncg);
@@ -197,11 +177,9 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
                 // slot / parity / addresses carried incrementally (the producer has to out-run the MMA issuer: no division, no call)
                 const uint32_t bar_wf = BAR(B_WFULL), bar_we = BAR(B_WEMPTY), dst0 = smem_u32(sW), nws_u = (uint32_t)NWS;
                 uint32_t sw = 0, ph = 1u, dst = dst0;
-                int wi = 0;
                 for (int g = 0; g < NG; g++) {
                     const uint8_t* src = wt;
-                    for (int cj = 0; cj < NCH * p.K; cj++, wi++, src += p.w_stage_bytes) {
-                        if ((p.dbg_flags & 4) && wi >= NWS) continue;
+                    for (int cj = 0; cj < NCH * p.K; cj++, src += p.w_stage_bytes) {
                         mbar_wait_u(bar_we + 8u * sw, ph);
                         mbar_expect_tx(bar_wf + 8u * sw, p.w_stage_bytes);
                         bulk_g2s(dst, src, p.w_stage_bytes, bar_wf + 8u * sw);
@@ -228,19 +206,19 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
         q.bar_af = BAR(B_AFULL); q.bar_ae = BAR(B_AEMPTY); q.bar_wf = BAR(B_WFULL); q.bar_we = BAR(B_WEMPTY); q.bar_acc = BAR(B_ACC);
         q.a_lo_base = ((smem_u32(sA) & 0x3ffffu) >> 4) | a_lo_c; q.w_lo_base = ((smem_u32(sW) & 0x3ffffu) >> 4) | b_lo_c;
         q.a_stage16 = p.a_stage_bytes >> 4; q.w_stage16 = p.w_stage_bytes >> 4;
-        q.a_kstep = a_kstep; q.b_kstep = b_kstep; q.nt = (uint32_t)nt; q.tapstep = (p.dbg_flags & 1) ? 0u : (uint32_t)p.dil; q.tm = tm;
+        q.a_kstep = a_kstep; q.b_kstep = b_kstep; q.nt = (uint32_t)nt; q.dil = (uint32_t)p.dil; q.tm = tm;
         q.nas = (uint32_t)NAS; q.nws = (uint32_t)NWS; q.NG = NG; q.NCH = NCH; q.K = p.K;
-        q.streamed = !p.resident; q.wcommit = q.streamed && !p.dbg_skip_wcommit; q.nostale = !(p.dbg_flags & 4);
+        q.streamed = !p.resident;
         q.hi = (uint64_t)desc_hi << 32;
-        if (nk == 2) g2_issuer_mg<2>(q, MG, prof, lane);
-        else g2_issuer_mg<1>(q, MG, prof, lane);  // g2_conv() admits KC = 16 or 32 only
+        if (nk == 2) g2_issuer_mg<2>(q, MG);
+        else g2_issuer_mg<1>(q, MG);  // g2_conv() admits KC = 16 or 32 only
     } else if (warp == 3) {
         // ===== zero halo of the OUTPUT tensor (= the conv padding of its consumers), written by its producer: the CTA of the first super-tile
         // clears rows [-G2_PADL, 0) if the window starts at t = 0, the CTA of the last one rows [T_out, T_out + G2_PADR) if the window ends at
         // T_out, for every channel group of batch b (N tile 0 only).  A window inside the tensor leaves the halo rows alone: in a streamed run
         // they are final rows of earlier windows.
         const bool lo = blockIdx.x == 0 && p.t_begin == 0, hi = blockIdx.x == gridDim.x - 1 && p.t_end == p.T;
-        if (!(p.dbg_flags & 16) && ntile == 0 && (lo || hi)) {
+        if (ntile == 0 && (lo || hi)) {
             asm volatile("griddepcontrol.wait;" ::: "memory");  // the rows may alias a tensor an upstream kernel is still reading
             uint4* yb = p.y + (size_t)b * p.y_cg * p.y_Tp;
             const int Tout = p.T * (p.ups_u ? p.ups_u : 1);
@@ -287,15 +265,7 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
         asm volatile("griddepcontrol.wait;" ::: "memory");
         const bool scaled = p.out_scale != 1.f;
         for (int g = 0; g < NG; g++) {
-            if (p.dbg_flags & 8) {
-                uint32_t done = 0;
-                while (!done) {
-                    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(done) : "r"(BAR(B_ACC + g)), "r"(0u) : "memory");
-                    if (!done) __nanosleep(2000);
-                }
-            } else mbar_wait(BAR(B_ACC + g), 0);
-            if (prof && e == 0 && lane == 0 && g == 0) prof[5] = gtime();
-            if (prof && e == 0 && lane == 0 && g == NG - 1) prof[6] = gtime();
+            mbar_wait(BAR(B_ACC + g), 0);
             for (int it = part; it < MG * ncb; it += 3) {
                 const int mt = it / ncb, col0 = (it - mt * ncb) * cw;
                 const int t = t0 + (g * MG + mt) * 128 + q * 32 + lane;
@@ -348,23 +318,7 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
             }
         }
     }
-    if (prof && warp == 4 && lane == 0) prof[7] = gtime();
     __syncthreads();
-}
-
-// ---- halo zeroing as a separate launch (probes; the engine's producers clear the halos of their own outputs, see k_g2_conv warp 3): the zero
-// rows around every H8 tensor are the conv padding of its consumers.  One launch per Generator stage
-// covers all tensors of the stage (the workspace is a bump arena: a stage's buffers alias whatever the previous call left there).
-struct G2HaloList { uint4* p[16]; int cg_rows[16]; int T[16]; int Tp[16]; int n; };  // cg_rows = B * C/8 channel-group runs
-__global__ void __launch_bounds__(128) k_g2_zero_halo(G2HaloList l) {
-    const int i = blockIdx.y;
-    if (i >= l.n) return;
-    const int per = G2_PADL + G2_PADR;
-    for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < l.cg_rows[i] * per; idx += gridDim.x * blockDim.x) {
-        const int run = idx / per, r = idx - run * per;
-        const int t = r < G2_PADL ? r - G2_PADL : l.T[i] + (r - G2_PADL);
-        l.p[i][(size_t)run * l.Tp[i] + t] = make_uint4(0u, 0u, 0u, 0u);
-    }
 }
 
 // fp32 c4 [B][C/4][T][4] (rows t >= lens[b] read as zero) -> raw f16 H8 (no activation): the Generator's input z * y_mask
@@ -436,10 +390,7 @@ struct G2Epi {
     const float* bias_b = nullptr; int bias_b_stride = 0;  // per-batch bias (speaker conditioning of conv_pre)
     int dil = 1;
     int t_begin = 0, t_end = -1;  // output window [t_begin, t_end) (t_end = -1: T_out); a ConvTranspose window is a multiple of its stride
-    int st_override = 0;      // probes: force the super-tile size (m-tiles per CTA)
-    long long* prof = nullptr;  // probes: per-CTA timestamps
-    int dbg_skip_wcommit = 0;
-    int dbg_flags = 0;
+    int st_override = 0;      // tests: force the super-tile size (m-tiles per CTA)
 };
 
 // Static part of the plan (fixed at weight-pack time): N tile and K chunk for a conv with `cols` output columns.
@@ -466,7 +417,7 @@ inline G2Plan g2_conv_plan(const TcConvW& w, const float* bias, const H8& x, con
     p.x = x.p; p.y = y.p; p.w = w.w; p.bias = bias; p.bias_b = e.bias_b; p.bias_b_stride = e.bias_b_stride;
     p.x_cg = x.C / 8; p.x_Tp = x.Tp; p.y_cg = y.C / 8; p.y_Tp = y.Tp;
     if (e.res) { BV2_CHECK(!w.ups_u && e.res->C == y.C && e.res->T == y.T && e.res->B == y.B, "g2_conv residual"); p.res = e.res->p; p.res_cg = e.res->C / 8; p.res_Tp = e.res->Tp; p.residual = 1; }
-    p.accumulate = e.accumulate; p.out_scale = e.out_scale; p.ups_u = w.ups_u; p.ups_cout = w.ups_cout; p.prof = e.prof; p.dbg_flags = e.dbg_flags;
+    p.accumulate = e.accumulate; p.out_scale = e.out_scale; p.ups_u = w.ups_u; p.ups_cout = w.ups_cout;
     if (w.ups_u) BV2_CHECK(w.ups_cout % 8 == 0 && !e.accumulate, "g2_conv ups");
     p.T = x.T; p.K = w.K; p.dil = e.dil; p.pad = (w.K - 1) / 2 * e.dil;
     BV2_CHECK(p.pad <= G2_PADL && p.pad <= G2_PADR, "g2_conv padding exceeds the tensor halo");
@@ -519,7 +470,6 @@ inline G2Plan g2_conv_plan(const TcConvW& w, const float* bias, const H8& x, con
     p.acc_cols = (uint32_t)(NG * MG * w.nt);
     const size_t smem = tc::acc_img_bytes(p.acc_cols) + (size_t)nas * p.a_stage_bytes + (p.resident ? w_all : (size_t)p.nws * p.w_stage_bytes) + (size_t)(2 * nas + 2 * p.nws + NG + 3) * 8 + 16;
     BV2_CHECK(smem <= 227 * 1024, "g2_conv shared memory");
-    if (e.dbg_skip_wcommit && !p.resident && p.nws >= NG * w.nchunks * w.K) p.dbg_skip_wcommit = 1;
     G2Plan pl;
     pl.resident = p.resident; pl.NG = NG; pl.MG = MG; pl.nas = nas; pl.nws = p.nws; pl.smem = smem;
     pl.grid = dim3(cdiv(mtiles, NG * MG), ntiles, x.B);

@@ -125,7 +125,7 @@ def attn_cases():
 
 # ---- Generator conv (k_g2_conv): (id, Cin, Cout, K, dil, u, T, B, res, acc, scale, st_override, bias_b)
 def g2_cases():
-    base = [  # every shape of the standalone probe: every tail, edge tiles, both weight modes
+    base = [  # the shape matrix: every tail, edge tiles, both weight modes
         (16, 16, 3, 1, 0, 300, 1, 0, 0, 1.0, 0), (16, 16, 11, 5, 0, 1000, 2, 1, 0, 1.0, 0), (16, 16, 7, 3, 0, 5000, 1, 1, 1, 1 / 3, 0),
         (32, 32, 11, 5, 0, 3000, 1, 1, 0, 1.0, 0), (32, 32, 3, 1, 0, 129, 3, 1, 1, 1.0, 0), (64, 64, 7, 3, 0, 2000, 1, 1, 0, 1.0, 0),
         (64, 64, 11, 1, 0, 700, 2, 0, 0, 1.0, 3), (128, 128, 3, 1, 0, 1000, 1, 1, 0, 1.0, 4), (128, 128, 11, 5, 0, 600, 1, 1, 1, 1 / 3, 2),

@@ -21,7 +21,7 @@ for r in rows[1:]:
     elif m.startswith("dram__bytes"): d["bytes"] += v * {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}.get(u, 1.0)
 ids = list(per)
 ends = [i for i in ids if per[i]["name"].startswith("k_conv_post_tanh")]
-starts = [i for i in ids if per[i]["name"].startswith(("k_c4_to_h8", "k_g2_zero_halo"))]
+starts = [i for i in ids if per[i]["name"].startswith("k_c4_to_h8")]
 end = ends[-1]
 start = max(i for i in starts if i < end and not any(e < end and e > i for e in ends))
 first = min(i for i in starts if i <= start and i > ([e for e in ends if e < end] or [-1])[-1])
