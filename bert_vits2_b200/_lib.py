@@ -42,6 +42,7 @@ P, I64P, F32P = C.c_void_p, C.c_void_p, C.c_void_p
 SYMBOLS = {
     "bv2_version": (C.c_char_p, []),
     "bv2_create": (C.c_int, [C.POINTER(P), C.POINTER(Bv2Config), C.c_int]),
+    "bv2_create_sibling": (C.c_int, [C.POINTER(P), P]),
     "bv2_set_weight": (C.c_int, [P, C.c_char_p, C.c_void_p, C.POINTER(C.c_int64), C.c_int, C.c_int]),
     "bv2_finalize": (C.c_int, [P]),
     "bv2_save_packed": (C.c_int, [P, C.c_char_p]),

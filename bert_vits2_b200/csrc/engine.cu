@@ -52,6 +52,8 @@ public:
     // Sticky high-water mark: the arena only ever grows, and when it must it grows to 1.5x the request (the frame count of an
     // utterance varies with the duration noise), so a steady workload allocates during its first call(s) and never again.
     // Regrowth is a device-wide sync + cudaFree + cudaMalloc; bv2_reserve() sizes the arenas up front so that serving loops never hit it.
+    // The sync also waits for the work of every other engine on the device (siblings included): correct, but a stall for them, so a
+    // server reserves each sibling too.
     void ensure(size_t bytes) {
         if (bytes <= cap_) return;
         bytes += bytes / 2;
@@ -76,22 +78,24 @@ private:
     void* base_ = nullptr; size_t cap_ = 0, off_ = 0; int grows_ = 0;
 };
 
+// One device error flag per device for the whole process.  tc_init_device() points the device-global g_tc_err_flag at a pinned int;
+// re-pointing it would leave every older engine reading a flag the device no longer raises, so the first finalize on a device creates
+// it, and it is never re-pointed or freed.  Every engine on the device reads the same flag: the first to see it raised consumes it
+// under g_err_mu (clears both flags) and bumps the generation.  Once g_tc_err_dev is set every in-flight wait on the device drains
+// early, so every call that was in flight at that moment has invalid results: a call fails if the generation changed since it began.
+struct DeviceErrFlag { int* host = nullptr; uint64_t generation = 0; };
+std::mutex g_err_mu;
+std::unordered_map<int, DeviceErrFlag> g_err_flags;
+
 }  // namespace bv2
 
 using namespace bv2;
 
-struct bv2_engine {
-    bv2_config cfg{};
-    int device = 0;
-    std::mutex mu;
-    std::string err;
-    std::unordered_map<std::string, HostTensor> host;
-    bool finalized = false;
-    std::vector<void*> dev_allocs;
-    int64_t launches = 0;
-    int num_sms = 132;
-
-    // ---- device weights
+// Everything finalize() builds that stays fixed afterwards: the device weight arena and the layout bookkeeping that points into it.
+// A sibling engine (bv2_create_sibling) copies this struct whole; the arena itself is shared and freed with the family's last member.
+struct DeviceWeights {
+    std::shared_ptr<uint8_t> warena_owner;
+    uint8_t* warena = nullptr; size_t warena_bytes = 0;
     float *emb = nullptr, *temb = nullptr, *lemb = nullptr, *emb_g = nullptr;
     ConvW bert_proj, enc_proj;
     EncoderW enc_p;
@@ -104,6 +108,22 @@ struct bv2_engine {
     float *gproj_w = nullptr, *gproj_b = nullptr; int gproj_n = 0;
     int goff_dec = 0, goff_sdp = 0, goff_dp = 0;
     float dconst = 0.f;
+    int hop = 512;
+    int flow_tc = 0;       // 0 SIMT fp32, 1 TF32 wgmma, 2 FP16 wgmma + fused attention (finalize)
+    int use_g2 = 0;        // FP16 Generator on 16-bit activation tensors (tc_gen.cuh)
+    std::vector<std::pair<std::string, std::vector<int64_t>>> shape_table;  // kept for bv2_save_packed
+};
+
+struct bv2_engine : DeviceWeights {
+    bv2_config cfg{};
+    int device = 0;
+    std::mutex mu;
+    std::string err;
+    std::unordered_map<std::string, HostTensor> host;
+    bool finalized = false;
+    int64_t launches = 0;
+    int num_sms = 132;
+    uint64_t call_gen = 0;  // device error generation when the current call began (check_device_error)
 
     // ---- workspace / per-call state
     Arena ws, persist;  // persist: state kept between infer_begin and infer_finish
@@ -129,8 +149,8 @@ struct bv2_engine {
         float* o = nullptr; const float* gdec = nullptr; int g_stride = 0; const int* lens = nullptr;
     } gs;
     void ws_reset() { gs.open = false; ws.reset(); }
-    long long* h_ylen = nullptr;  // pinned
-    int* h_err = nullptr;         // pinned + mapped: device-side error flag (barrier timeouts), see tc_conv.cuh
+    long long* h_ylen = nullptr;  // pinned: y_lengths[B <= 4096] + the input-validation mask
+    void ensure_h_ylen() { if (!h_ylen) BV2_CUDA(cudaMallocHost(&h_ylen, 4100 * sizeof(long long))); }
     // side streams: the MRF's resblocks (k = 3, 7, 11) of one Generator stage are independent chains of 6 convs
     cudaStream_t side[4] = {nullptr, nullptr, nullptr, nullptr};
     cudaEvent_t ev_fork = nullptr, ev_rb[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -139,8 +159,6 @@ struct bv2_engine {
         for (int i = 0; i < 4; i++) { BV2_CUDA(cudaStreamCreateWithFlags(&side[i], cudaStreamNonBlocking)); BV2_CUDA(cudaEventCreateWithFlags(&ev_rb[i], cudaEventDisableTiming)); }
         BV2_CUDA(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
     }
-    int flow_tc = 0;       // 0 SIMT fp32, 1 TF32 wgmma, 2 FP16 wgmma + fused attention (finalize)
-    int use_g2 = 0;        // FP16 Generator on 16-bit activation tensors (tc_gen.cuh)
     bool profiling = false;
     struct StageEv { cudaEvent_t a = nullptr, b = nullptr; bool rec = false; };
     std::map<std::string, StageEv> stage_ev;
@@ -157,10 +175,7 @@ struct bv2_engine {
     }
 
     ~bv2_engine() {
-        for (void* p : dev_allocs) cudaFree(p);
-        if (warena) cudaFree(warena);
         if (h_ylen) cudaFreeHost(h_ylen);
-        if (h_err) cudaFreeHost(h_err);
         for (int i = 0; i < 4; i++) { if (side[i]) cudaStreamDestroy(side[i]); if (ev_rb[i]) cudaEventDestroy(ev_rb[i]); }
         if (ev_fork) cudaEventDestroy(ev_fork);
         for (auto& kv : stage_ev) { if (kv.second.a) cudaEventDestroy(kv.second.a); if (kv.second.b) cudaEventDestroy(kv.second.b); }
@@ -176,7 +191,7 @@ struct bv2_engine {
     // lives in ONE allocation filled by ONE cudaMemcpy.  build_weights() runs twice: a measuring pass (sizes only, packing
     // loops skipped) and the real pass that writes into a host mirror at the same offsets.  bv2_save_packed() dumps that
     // arena; bv2_load_packed() re-runs the structure pass with the packing loops skipped and copies the file in (SURVEY 8f.4).
-    uint8_t* warena = nullptr; size_t warena_bytes = 0, woff = 0;
+    size_t woff = 0;
     std::vector<uint8_t> wmirror;
     bool wmeasure = false, wfill = true;
     bool packing() const { return wfill && !wmeasure; }  // false: skip the expensive fold / repack loops (only sizes matter)
@@ -303,7 +318,6 @@ struct bv2_engine {
         enc_p = EncoderW(); sdp_dds = DdsW(); sdp_flows.clear(); flows.clear(); ups.clear(); resblocks.clear();
         bert_proj = enc_proj = sdp_pre = sdp_proj = dp_c1 = dp_c2 = dp_proj = conv_pre = ConvW();
     }
-    std::vector<std::pair<std::string, std::vector<int64_t>>> shape_table;  // kept for bv2_save_packed
 
     // ---------------------------------------------------------------- launch helpers
     int tc_out_tf32 = 0, tc_skip_xform = 0, tc_in_f16 = 0, tc_out_f16 = 0;  // one-shot modifiers for the next tensor-core conv() call
@@ -420,7 +434,6 @@ struct bv2_engine {
         BV2_CUDA(cudaStreamSynchronize(s));
         throw_if_bad_inputs(h);
     }
-    int hop = 512;
     // wave [B][L] fp32 -> int16 (peak-normalised per utterance over n_valid samples; ylen given in units of `unit` samples)
     void pcm16(const float* wave, int B, long long L, const long long* ylen, int unit, long long* nval_scratch, unsigned* peak, int16_t* out, cudaStream_t s) {
         const long long* nv = ylen;
@@ -435,12 +448,20 @@ struct bv2_engine {
         k_wave_to_pcm16<<<g2, 256, 0, s>>>(wave, L, nv, peak, reinterpret_cast<short*>(out));
         BV2_CUDA(cudaGetLastError()); launches += 2;
     }
+    void begin_call() {
+        std::lock_guard<std::mutex> lk(g_err_mu);
+        call_gen = g_err_flags[device].generation;
+    }
     void check_device_error() {
-        if (h_err && *reinterpret_cast<volatile int*>(h_err)) {
-            *h_err = 0;
+        std::lock_guard<std::mutex> lk(g_err_mu);
+        DeviceErrFlag& f = g_err_flags[device];
+        if (f.host && *reinterpret_cast<volatile int*>(f.host)) {
+            *f.host = 0;
             tc_clear_error();
-            throw Error(BV2_ERR_INTERNAL, "device-side barrier timeout in a wgmma kernel (results of this call are invalid)");
+            f.generation++;
         }
+        if (f.generation != call_gen)
+            throw Error(BV2_ERR_INTERNAL, "device-side barrier timeout in a wgmma kernel on this device (results of this call are invalid)");
     }
 };
 
@@ -470,7 +491,11 @@ void bv2_engine::finalize(const uint8_t* packed, size_t packed_bytes) {
     BV2_CHECK(c.n_flows >= 1 && c.n_flows <= 16, "n_flows");
     BV2_CHECK(c.sdp_num_bins == 10 && c.sdp_kernel == 3, "sdp spline bins/kernel");
     BV2_CUDA(cudaSetDevice(device));
-    if (!h_err) h_err = tc_init_device();  // > 48 KB dynamic shared memory opt-in (a per-device function attribute) + device error flag
+    {   // > 48 KB dynamic shared memory opt-in (a per-device function attribute) + the device error flag: once per device and process
+        std::lock_guard<std::mutex> lk(g_err_mu);
+        DeviceErrFlag& f = g_err_flags[device];
+        if (!f.host) f.host = tc_init_device();
+    }
     tok_init_device();
     shape_table.clear();
     for (const auto& kv : host) shape_table.emplace_back(kv.first, kv.second.shape);
@@ -481,6 +506,7 @@ void bv2_engine::finalize(const uint8_t* packed, size_t packed_bytes) {
     const size_t total = woff;
     reset_weights();
     BV2_CUDA(cudaMalloc(reinterpret_cast<void**>(&warena), total));
+    warena_owner.reset(warena, [](uint8_t* p) { cudaFree(p); });
     warena_bytes = total;
     wmeasure = false; woff = 0;
     if (packed) {
@@ -495,7 +521,7 @@ void bv2_engine::finalize(const uint8_t* packed, size_t packed_bytes) {
         BV2_CUDA(cudaMemcpy(warena, wmirror.data(), total, cudaMemcpyHostToDevice));
         std::vector<uint8_t>().swap(wmirror);
     }
-    if (!h_ylen) BV2_CUDA(cudaMallocHost(&h_ylen, 4100 * sizeof(long long)));
+    ensure_h_ylen();
     if (use_g2) {  // same bytes whichever way the arena was filled (state_dict or packed file)
         BV2_CHECK(c.upsample_initial_channel >> c.n_ups == 16, "conv_post kernel instantiated for 16 input channels, 7 taps");
         BV2_CUDA(cudaMemcpy(conv_post_h.w, conv_post_w, sizeof(conv_post_h.w), cudaMemcpyDeviceToHost));
@@ -1218,7 +1244,8 @@ void bv2_engine::g2_windows(const GenGraph& g, const std::vector<GenWin>& w, std
     if (!(e)) return BV2_ERR_ARG;                         \
     std::lock_guard<std::mutex> _lk((e)->mu);             \
     try {                                                 \
-        BV2_CUDA(cudaSetDevice((e)->device));
+        BV2_CUDA(cudaSetDevice((e)->device));             \
+        (e)->begin_call();
 #define BV2_API_END(e)                                    \
     }                                                     \
     catch (const bv2::Error& ex) { (e)->err = ex.what(); return ex.code; } \
@@ -1256,6 +1283,25 @@ int bv2_create(bv2_engine** out, const bv2_config* cfg, int cuda_device) {
     e->device = cuda_device;
     e->num_sms = prop.multiProcessorCount;
     *out = e;
+    return BV2_OK;
+}
+
+int bv2_create_sibling(bv2_engine** out, bv2_engine* src) {
+    if (!out || !src) return BV2_ERR_ARG;
+    *out = nullptr;
+    std::lock_guard<std::mutex> lk(src->mu);
+    if (!src->finalized) { src->err = "create_sibling needs a finalized engine (bv2_finalize or bv2_load_packed)"; return BV2_ERR_STATE; }
+    std::unique_ptr<bv2_engine> e(new bv2_engine());
+    e->cfg = src->cfg;
+    e->device = src->device;
+    e->num_sms = src->num_sms;
+    static_cast<DeviceWeights&>(*e) = static_cast<const DeviceWeights&>(*src);
+    e->finalized = true;  // bv2_set_weight / bv2_finalize / bv2_load_packed return BV2_ERR_STATE on a sibling
+    try {
+        BV2_CUDA(cudaSetDevice(e->device));
+        e->ensure_h_ylen();
+    } catch (const bv2::Error& ex) { src->err = ex.what(); return ex.code; }
+    *out = e.release();
     return BV2_OK;
 }
 

@@ -51,7 +51,7 @@ def _ptr(t: Optional[torch.Tensor]):
 
 
 class Engine:
-    """One engine per CUDA device.  precision: 'fp32' (SIMT FMA everywhere), 'tf32' (wgmma implicit-GEMM convs with TF32
+    """An engine on one CUDA device; it serves one request at a time (sibling() gives another over the same weights).  precision: 'fp32' (SIMT FMA everywhere), 'tf32' (wgmma implicit-GEMM convs with TF32
     operands) or 'fp16' (wgmma with FP16 operands -- same 11-bit significand as TF32, twice the tensor rate, half the
     operand traffic; fp32 accumulate and fp32 activations in HBM).  Everything that feeds ceil(durations) is FP32 FMA in all three."""
 
@@ -84,6 +84,20 @@ class Engine:
             shape = (C.c_int64 * max(1, t.dim()))(*t.shape)
             self._check(self.lib.bv2_set_weight(self._h, k.encode(), C.c_void_p(t.data_ptr()), shape, t.dim(), dt))
         self._check(self.lib.bv2_finalize(self._h))
+
+    def sibling(self) -> "Engine":
+        """A second engine over this engine's device weights (bv2_create_sibling: nothing is copied).  It has its own workspace,
+        per-call state and mutex, so it can serve a request on another CUDA stream while this one serves another."""
+        sib = Engine.__new__(Engine)
+        sib.lib, sib.cfg, sib.device, sib.precision = self.lib, self.cfg, self.device, self.precision
+        sib._h = C.c_void_p()
+        self._check(self.lib.bv2_create_sibling(C.byref(sib._h), self._h))
+        return sib
+
+    @property
+    def workspace_bytes(self) -> int:
+        """Bytes of workspace (both arenas) this engine holds."""
+        return int(self.lib.bv2_workspace_bytes(self._h))
 
     def save_packed(self, path: str):
         """Dump the finalized weight arena (folded + packed for this config and precision); reload with Engine(cfg, None, packed_path=path)."""

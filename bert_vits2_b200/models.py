@@ -15,6 +15,8 @@ CPU fallback — calling .infer() on a CPU module raises.
 """
 from __future__ import annotations
 
+import contextlib
+import threading
 from typing import Optional
 
 import torch
@@ -22,22 +24,61 @@ from torch import nn
 
 from . import synth
 from .engine import Bv2Error, Engine
+from .pool import EnginePool
 from .spec import ModelConfig, param_specs
+
+_ENGINE_LOCK = threading.Lock()  # builds a module's engine and pool once when several threads make its first call together
+
+
+class _Lane:
+    """Where a leased engine's work runs.  Without an own stream (concurrency=1): on the caller's current stream, as a single engine
+    always ran.  With one: on the engine's own stream, which waits for the caller's work before each step; after the step the caller's
+    stream waits for it, and every result tensor is recorded on the caller's stream so that the caching allocator does not hand its
+    memory to the engine's next request while the caller still reads it."""
+
+    def __init__(self, eng, own_stream: bool):
+        self.stream = None
+        if own_stream:
+            if getattr(eng, "serve_stream", None) is None:
+                eng.serve_stream = torch.cuda.Stream(eng.device)
+            self.stream, self.caller = eng.serve_stream, torch.cuda.current_stream(eng.device)
+
+    @contextlib.contextmanager
+    def step(self):
+        """Yields a list: append the step's result tensors to it."""
+        results = []
+        if self.stream is None:
+            yield results
+            return
+        self.stream.wait_stream(self.caller)
+        try:
+            with torch.cuda.stream(self.stream):
+                yield results
+        finally:
+            self.caller.wait_stream(self.stream)
+        for t in results:
+            if t is not None:
+                t.record_stream(self.caller)
 
 
 class LazyAttn:
     """Stand-in for the `attn` tensor infer() returns (reference models.py:1074): the dense [B,1,F,T] one-hot path is only
     written when somebody reads it (the reference's own callers never do: infer.py:302-318 uses `o` alone).  Any attribute
-    access, indexing or torch function materialises it once through bv2_attn_path; `.materialize()` returns the tensor."""
+    access, indexing or torch function materialises it once through bv2_attn_path; `.materialize()` returns the tensor.
+    Materialising leases the engine that served the call, and raises if that engine has served another request since."""
 
-    def __init__(self, engine, shape, token):
-        self._engine, self._shape, self._token, self._t = engine, tuple(shape), token, None
+    def __init__(self, engine, shape, token, pool: EnginePool):
+        self._engine, self._shape, self._token, self._pool, self._t = engine, tuple(shape), token, pool, None
 
     def materialize(self) -> torch.Tensor:
         if self._t is None:
-            if getattr(self._engine, "_attn_token", None) is not self._token:
-                raise RuntimeError("attn of an earlier infer() call: materialise it before the next call on the same module")
-            self._t = self._engine.attn_path()
+            with self._pool.lease(self._engine) as eng:
+                if getattr(eng, "_attn_token", None) is not self._token:
+                    raise RuntimeError("attn of an earlier infer() call: materialise it before the engine that served it serves the next "
+                                       "request (with concurrency=1: before the next call on the same module)")
+                with _Lane(eng, self._pool.concurrency > 1).step() as results:
+                    self._t = eng.attn_path()
+                    results.append(self._t)
         return self._t
 
     @property
@@ -79,8 +120,10 @@ class SynthesizerTrn(nn.Module):
                  n_layers, kernel_size, p_dropout, resblock, resblock_kernel_sizes, resblock_dilation_sizes, upsample_rates,
                  upsample_initial_channel, upsample_kernel_sizes, n_speakers=256, gin_channels=256, use_sdp=True,
                  n_flow_layer=4, n_layers_trans_flow=4, flow_share_parameter=False, use_transformer_flow=True,
-                 precision: str = "fp16", init_seed: Optional[int] = 0, **kwargs):
+                 precision: str = "fp16", init_seed: Optional[int] = 0, concurrency: int = 1, **kwargs):
         super().__init__()
+        if int(concurrency) < 1:
+            raise ValueError("concurrency must be >= 1")
         if n_speakers < 1:
             raise ValueError("n_speakers == 0 (ReferenceEncoder path, models.py:752-808) is a training-only configuration")
         if flow_share_parameter:
@@ -92,6 +135,8 @@ class SynthesizerTrn(nn.Module):
         self.n_heads, self.n_layers, self.kernel_size, self.p_dropout = n_heads, n_layers, kernel_size, p_dropout
         self.n_speakers, self.gin_channels, self.use_sdp = n_speakers, gin_channels, use_sdp
         self.precision = precision
+        self.concurrency = int(concurrency)
+        self._tls = threading.local()
         model = dict(inter_channels=inter_channels, hidden_channels=hidden_channels, filter_channels=filter_channels,
                      n_heads=n_heads, n_layers=n_layers, kernel_size=kernel_size, resblock=resblock,
                      resblock_kernel_sizes=list(resblock_kernel_sizes),
@@ -111,13 +156,24 @@ class SynthesizerTrn(nn.Module):
             t = init[p.key] if init is not None else torch.zeros(p.shape)
             node.register_parameter(parts[-1], nn.Parameter(t, requires_grad=False))
         self._engines = {}
+        self._pools = {}
         self._weights_version = 0
         self.register_load_state_dict_post_hook(lambda module, incompatible: module._invalidate())
+
+    @property
+    def last_y_lengths(self):
+        """y_lengths of the calling thread's latest infer() / infer_stream() (each thread reads its own request's)."""
+        return self._tls.y_lengths
+
+    @last_y_lengths.setter
+    def last_y_lengths(self, v):
+        self._tls.y_lengths = v
 
     # -- weight changes invalidate the packed device copy ------------------------------------------------
     def _invalidate(self):
         self._weights_version += 1
         self._engines.clear()
+        self._pools.clear()
 
     def _apply(self, fn, *a, **kw):
         r = super()._apply(fn, *a, **kw)
@@ -137,6 +193,23 @@ class SynthesizerTrn(nn.Module):
             self._engines = {key: eng}
         return eng
 
+    def _pool(self, device: torch.device) -> EnginePool:
+        """The engine pool of `device`: the primary engine of _engine() plus up to concurrency - 1 siblings, created when needed."""
+        with _ENGINE_LOCK:
+            eng = self._engine(device)
+            key = (str(device), self._weights_version)
+            pool = self._pools.get(key)
+            if pool is None or pool.primary is not eng:
+                pool = EnginePool(eng, self.concurrency, lambda primary: primary.sibling())
+                self._pools = {key: pool}
+            return pool
+
+    def _cuda_device(self, what: str) -> torch.device:
+        dev = next(self.parameters()).device
+        if dev.type != "cuda":
+            raise Bv2Error(f"SynthesizerTrn.{what}: module is on CPU; bert_vits2_b200 has no CPU path — call .to('cuda')")
+        return dev
+
     # ----------------------------------------------------------------------------------------------------
     @torch.no_grad()
     def infer(self, x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_scale=0.667, length_scale=1,
@@ -144,24 +217,26 @@ class SynthesizerTrn(nn.Module):
         """reference models.py:1026-1074.  Keyword-only extras (not in the reference): explicit noise tensors
         `noise_w` [B,2,T] / `noise_z` [B,inter,>=F] replacing the two in-model RNG draws (models.py:249, 1071), and
         `w_ceil_override` [B,T] to teacher-force durations in parity harnesses, `pcm16=True` to get `o` as int16 converted like
-        the reference's callers do (gradio convert_to_16_bit_wav, webui.py:86).  `attn` comes back as a LazyAttn (see above)."""
-        dev = next(self.parameters()).device
-        if dev.type != "cuda":
-            raise Bv2Error("SynthesizerTrn.infer: module is on CPU; bert_vits2_b200 has no CPU path — call .to('cuda')")
+        the reference's callers do (gradio convert_to_16_bit_wav, webui.py:86).  `attn` comes back as a LazyAttn (see above).
+        The call leases one engine of the module's pool from begin to finish (concurrency=N: up to N calls run at once)."""
+        dev = self._cuda_device("infer")
         if x.dim() != 2 or bert.dim() != 3 or bert.shape[-1] != x.shape[1]:
             raise ValueError("expected x [B,T] and bert features [B,1024,T]")
-        eng = self._engine(dev)
+        pool = self._pool(dev)
         B, T = x.shape
-        if noise_w is None:  # same draw order/shape as the reference: SDP first (models.py:249)
-            noise_w = torch.randn(B, 2, T, device=dev, dtype=torch.float32)
-        y_lengths, F = eng.infer_begin(x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_w, noise_scale_w,
-                                       length_scale, sdp_ratio, w_ceil_override)
-        if noise_z is None:  # torch.randn_like(m_p), m_p: [B, inter, F] (models.py:1071)
-            noise_z = torch.randn(B, self.inter_channels, F, device=dev, dtype=torch.float32)
-        o, _, y_mask, aux = eng.infer_finish(B, T, F, noise_z, noise_scale, max_len, want_attn=False, pcm16=pcm16)
-        eng._attn_token = token = object()
+        with pool.lease() as eng:
+            with _Lane(eng, self.concurrency > 1).step() as results:
+                if noise_w is None:  # same draw order/shape as the reference: SDP first (models.py:249)
+                    noise_w = torch.randn(B, 2, T, device=dev, dtype=torch.float32)
+                y_lengths, F = eng.infer_begin(x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_w, noise_scale_w,
+                                               length_scale, sdp_ratio, w_ceil_override)
+                if noise_z is None:  # torch.randn_like(m_p), m_p: [B, inter, F] (models.py:1071)
+                    noise_z = torch.randn(B, self.inter_channels, F, device=dev, dtype=torch.float32)
+                o, _, y_mask, aux = eng.infer_finish(B, T, F, noise_z, noise_scale, max_len, want_attn=False, pcm16=pcm16)
+                results += [o, y_mask, *aux]
+            eng._attn_token = token = object()
         self.last_y_lengths = y_lengths
-        return o, LazyAttn(eng, (B, 1, F, T), token), y_mask, aux
+        return o, LazyAttn(eng, (B, 1, F, T), token, pool), y_mask, aux
 
     @torch.no_grad()
     def infer_stream(self, x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_scale=0.667, length_scale=1,
@@ -172,36 +247,43 @@ class SynthesizerTrn(nn.Module):
         attention spans the utterance); the Generator then runs as a wavefront, so the first chunk costs about first_chunk_frames
         + 14 frames of Generator work instead of all of it.  Chunks are first_chunk_frames frames, then double.  Each chunk is final
         when it is yielded (the host waits on an event recorded after its work) and no later chunk writes it.  Noise is drawn exactly
-        as infer() draws it.  `last_y_lengths` is set before the first chunk.  There is no pcm16 option: the PCM conversion normalises by the peak of the whole utterance."""
-        dev = next(self.parameters()).device
-        if dev.type != "cuda":
-            raise Bv2Error("SynthesizerTrn.infer_stream: module is on CPU; bert_vits2_b200 has no CPU path — call .to('cuda')")
+        as infer() draws it.  `last_y_lengths` is set before the first chunk.  There is no pcm16 option: the PCM conversion normalises by the peak of the whole utterance.
+        The generator leases one engine of the module's pool from its first step until it is exhausted, closed or collected."""
+        dev = self._cuda_device("infer_stream")
         if x.dim() != 2 or bert.dim() != 3 or bert.shape[-1] != x.shape[1]:
             raise ValueError("expected x [B,T] and bert features [B,1024,T]")
         if first_chunk_frames < 1:
             raise ValueError("first_chunk_frames must be >= 1")
-        eng = self._engine(dev)
+        pool = self._pool(dev)
         B, T = x.shape
-        if noise_w is None:
-            noise_w = torch.randn(B, 2, T, device=dev, dtype=torch.float32)
-        y_lengths, F = eng.infer_begin(x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_w, noise_scale_w,
-                                       length_scale, sdp_ratio, w_ceil_override)
-        if noise_z is None:
-            noise_z = torch.randn(B, self.inter_channels, F, device=dev, dtype=torch.float32)
-        o, _, _, _ = eng.infer_finish_stream(B, T, F, noise_z, noise_scale, max_len, want_attn=False)
-        eng._attn_token = object()  # a LazyAttn of an earlier infer() must not materialise this utterance's path
-        self.last_y_lengths = y_lengths
-        hop = self.cfg.hop
-        Fg = o.shape[-1] // hop
-        done, step = 0, int(first_chunk_frames)
-        while done < Fg:
-            target = min(done + step, Fg)
-            eng.stream_advance(target)
-            ev = torch.cuda.Event()
-            ev.record(torch.cuda.current_stream(dev))
-            ev.synchronize()
-            yield o[:, :, done * hop:target * hop]
-            done, step = target, 2 * step
+        eng = pool.acquire()
+        try:
+            lane = _Lane(eng, self.concurrency > 1)
+            with lane.step() as results:
+                if noise_w is None:
+                    noise_w = torch.randn(B, 2, T, device=dev, dtype=torch.float32)
+                y_lengths, F = eng.infer_begin(x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_w, noise_scale_w,
+                                               length_scale, sdp_ratio, w_ceil_override)
+                if noise_z is None:
+                    noise_z = torch.randn(B, self.inter_channels, F, device=dev, dtype=torch.float32)
+                o, _, _, _ = eng.infer_finish_stream(B, T, F, noise_z, noise_scale, max_len, want_attn=False)
+                results.append(o)
+            eng._attn_token = object()  # a LazyAttn of an earlier infer() must not materialise this utterance's path
+            self.last_y_lengths = y_lengths
+            hop = self.cfg.hop
+            Fg = o.shape[-1] // hop
+            done, step = 0, int(first_chunk_frames)
+            while done < Fg:
+                target = min(done + step, Fg)
+                with lane.step():
+                    eng.stream_advance(target)
+                    ev = torch.cuda.Event()
+                    ev.record(torch.cuda.current_stream(dev))
+                    ev.synchronize()
+                yield o[:, :, done * hop:target * hop]
+                done, step = target, 2 * step
+        finally:
+            pool.release(eng)
 
     def forward(self, *a, **kw):
         raise NotImplementedError("training forward (reference models.py:937-1024) is out of scope; use .infer()")

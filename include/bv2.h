@@ -11,7 +11,9 @@
  * [B,C,T]); the engine owns weights and workspace.  Work is enqueued on the caller's `stream`
  * (a cudaStream_t passed as void*); the only host synchronisation is inside bv2_infer_begin (one read-back of
  * y_lengths, the same data-dependent length the reference syncs on at models.py:1058 / commons.py:120-121).
- * One engine per device; concurrent callers are serialised by an internal mutex (ctypes drops the GIL).
+ * Calls on one engine are serialised by its internal mutex (ctypes drops the GIL), but a request spans two calls
+ * (bv2_infer_begin .. bv2_infer_finish*, or a stream up to its last bv2_stream_advance), so one engine serves one request at a
+ * time.  To serve several at once, give each its own sibling engine (bv2_create_sibling) and its own CUDA stream.
  * There is NO CPU fallback: creation fails if no sm_90 (H100) device is present.
  */
 #ifndef BV2_H_
@@ -59,6 +61,17 @@ typedef struct {
 
 /* replaces: models.SynthesizerTrn(...).to(device) (reference infer.py:95-101) */
 int bv2_create(bv2_engine** out, const bv2_config* cfg, int cuda_device);
+
+/* A sibling shares the finalized device weights of `src` (nothing is copied or re-packed) and owns everything a call writes: workspace
+ * arenas, per-call state (infer_begin..finish, open Generator stream, attn path, debug taps), pinned read-back buffer, side streams and
+ * events, profiling events, launch/grow counters, error text and its own mutex.  Calls on different members of a family do not
+ * serialise on the host and may run concurrently on different CUDA streams; their outputs are bit-identical to those of `src`.
+ * `src` must be finalized (bv2_finalize or bv2_load_packed), else BV2_ERR_STATE.  A sibling of a sibling joins the same family.
+ * bv2_set_weight, bv2_finalize and bv2_load_packed on a sibling return BV2_ERR_STATE; bv2_save_packed works on any member.  The device
+ * weights are reference-counted: freed with the family's last member, in any destruction order.  A sibling starts with an empty
+ * workspace (bv2_workspace_bytes == 0); a workspace regrowth synchronises the device and so stalls the other members' work:
+ * bv2_reserve each sibling up front. */
+int bv2_create_sibling(bv2_engine** out, bv2_engine* src);
 
 /* replaces: load_state_dict for one entry of `G_*.pth["model"]` (reference utils.py:65-120).
  * `key` is the reference state_dict key (weight-norm as weight_g/weight_v); host_ptr is HOST memory;
