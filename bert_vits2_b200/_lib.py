@@ -19,6 +19,9 @@ HARNESS_PATH = os.path.join(HERE, "libbv2_kernel_harness.so")
 # streaming harness (tests/cuda/stream_harness.cu): the Generator's window launches and wavefront planner, on top of the kernel harness
 STREAM_HARNESS_SOURCE = os.path.join(ROOT, "tests", "cuda", "stream_harness.cu")
 STREAM_HARNESS_PATH = os.path.join(HERE, "libbv2_stream_harness.so")
+# bounded-stream harness (tests/cuda/stream_bounded_harness.cu): the resident-range planner and launches, on top of the kernel harness
+BOUNDED_HARNESS_SOURCE = os.path.join(ROOT, "tests", "cuda", "stream_bounded_harness.cu")
+BOUNDED_HARNESS_PATH = os.path.join(HERE, "libbv2_stream_bounded_harness.so")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
 MAX_UPS, MAX_RK, MAX_DIL = 8, 4, 4
@@ -53,9 +56,13 @@ SYMBOLS = {
     "bv2_infer_finish_pcm16": (C.c_int, [P, F32P, C.c_int64, C.c_float, C.c_int32, C.c_void_p, F32P, F32P, F32P, F32P, F32P, F32P, C.c_void_p]),
     "bv2_infer_finish_stream": (C.c_int, [P, F32P, C.c_int64, C.c_float, C.c_int32, F32P, F32P, F32P, F32P, F32P, F32P, F32P, C.c_void_p]),
     "bv2_stream_advance": (C.c_int, [P, C.c_int32, C.c_void_p, C.POINTER(C.c_int64)]),
+    "bv2_infer_finish_stream_bounded": (C.c_int, [P, F32P, C.c_int64, C.c_float, C.c_int32, C.c_int32, F32P, F32P, F32P, F32P, F32P, F32P, F32P,
+                                                  C.c_void_p]),
+    "bv2_stream_bytes": (C.c_int64, [P, C.c_int, C.c_int32, C.c_int32]),
     "bv2_wave_to_pcm16": (C.c_int, [P, C.c_int, C.c_int64, F32P, I64P, C.c_void_p, C.c_void_p]),
     "bv2_attn_path": (C.c_int, [P, F32P, C.c_void_p]),
     "bv2_reserve": (C.c_int, [P, C.c_int, C.c_int, C.c_int]),
+    "bv2_reserve_stream": (C.c_int, [P, C.c_int, C.c_int, C.c_int, C.c_int32]),
     "bv2_text_encoder": (C.c_int, [P, C.c_int, C.c_int, I64P, I64P, I64P, I64P, I64P, F32P, F32P, F32P, F32P, F32P, F32P, C.c_void_p]),
     "bv2_duration": (C.c_int, [P, C.c_int, C.c_int, F32P, I64P, I64P, F32P, C.c_float, F32P, F32P, C.c_void_p]),
     "bv2_flow_reverse": (C.c_int, [P, C.c_int, C.c_int, F32P, I64P, I64P, F32P, C.c_void_p]),
@@ -104,20 +111,28 @@ def build(force: bool = False, verbose: bool = False) -> str:
         return LIB_PATH
 
 
-def harness_needs_build(stream: bool = False) -> bool:
-    path = STREAM_HARNESS_PATH if stream else HARNESS_PATH
+def _harness(stream: bool, bounded: bool):
+    """(source, library) of a test harness"""
+    if bounded:
+        return BOUNDED_HARNESS_SOURCE, BOUNDED_HARNESS_PATH
+    return (STREAM_HARNESS_SOURCE, STREAM_HARNESS_PATH) if stream else (HARNESS_SOURCE, HARNESS_PATH)
+
+
+def harness_needs_build(stream: bool = False, bounded: bool = False) -> bool:
+    src, path = _harness(stream, bounded)
     if not os.path.isfile(path):
         return True
     t = os.path.getmtime(path)
-    deps = [HARNESS_SOURCE] + ([STREAM_HARNESS_SOURCE] if stream else []) + HEADERS
+    deps = {HARNESS_SOURCE, src} | set(HEADERS)
     return any(os.path.getmtime(p) > t for p in deps if os.path.isfile(p))
 
 
-def build_harness(force: bool = False, stream: bool = False) -> str:
-    """Compile the kernel test harness (stream=True: the streaming harness) next to libbv2.so with the product flags."""
-    src, path = (STREAM_HARNESS_SOURCE, STREAM_HARNESS_PATH) if stream else (HARNESS_SOURCE, HARNESS_PATH)
+def build_harness(force: bool = False, stream: bool = False, bounded: bool = False) -> str:
+    """Compile the kernel test harness (stream=True: the streaming harness, bounded=True: the bounded-stream harness) next to
+    libbv2.so with the product flags."""
+    src, path = _harness(stream, bounded)
     with _lock:
-        if not force and not harness_needs_build(stream):
+        if not force and not harness_needs_build(stream, bounded):
             return path
         tmp = path + ".tmp"
         r = subprocess.run(["nvcc"] + NVCC_FLAGS + ["-o", tmp, src], capture_output=True, text=True)

@@ -143,10 +143,16 @@ struct bv2_engine : DeviceWeights {
     //   fp32 / TF32 Generator (fp32 c4):     4 * (512 + 17 * (256*8 + 128*64 + 64*128 + 32*256 + 16*512))       = 2,369,536 bytes.
     // The stream also reads the per-batch conditioning and the lengths in the persist arena.  Any call that resets the workspace, and a
     // bv2_reserve that regrows either arena, closes the stream.
+    // A bounded stream (FP16 Generator, chunks of at most max_chunk frames < Fg) keeps only the rows later windows still read: every
+    // H8 tensor, the input included, has gen_stream_capacity() rows of storage, independent of Fg, and a slide (k_g2_slide) moves a
+    // tensor's live rows to the front of its storage when a chunk would run past its end.  The input is converted from z chunk by chunk.
     struct {
         bool open = false; int B = 0, Fg = 0, frontier = 0;
         GenGraph g; std::vector<H8> t; std::vector<Act> a;  // tensors of the FP16 Generator (t) / of the fp32 c4 Generator (a)
         float* o = nullptr; const float* gdec = nullptr; int g_stride = 0; const int* lens = nullptr;
+        int max_chunk = 0;     // > 0: bounded stream
+        std::vector<int> cap;  // bounded: rows of storage per tensor (gen_stream_capacity)
+        Act z; const int* zlens = nullptr;  // bounded: the Generator input z (fp32 c4) and its lengths, converted per chunk
     } gs;
     void ws_reset() { gs.open = false; ws.reset(); }
     long long* h_ylen = nullptr;  // pinned: y_lengths[B <= 4096] + the input-validation mask
@@ -394,11 +400,14 @@ struct bv2_engine : DeviceWeights {
     void run_flow(Act z, const int* lens, const float* gproj, cudaStream_t s);
     void run_generator(Act z, const int* lens_or_null, const float* gdec, int g_stride, float* o, cudaStream_t s);
     void run_generator_g2(Act z, const int* lens_or_null, const float* gdec, int g_stride, float* o, cudaStream_t s);
-    H8 g2_h8(int B, int C, int T);
+    H8 g2_h8(int B, int C, int T, int rows = -1);
     H8 g2_input(Act z, const int* lens_or_null, cudaStream_t s);
     int gen_channels(const GenGraph& g, int tensor) const;
     size_t gen_stream_bytes(int B, int Fg) const;
-    void gen_stream_open(Act z, const int* lens_or_null, const float* gdec, int g_stride, float* o, cudaStream_t s);
+    bool stream_bounded(int Fg, int max_chunk) const { return use_g2 && max_chunk >= 1 && max_chunk < Fg; }
+    size_t stream_bytes(int B, int Fg, int max_chunk) const;
+    void gen_stream_open(Act z, const int* lens_or_null, const float* gdec, int g_stride, float* o, int max_chunk, cudaStream_t s);
+    void g2_stream_prepare(int done, int target, cudaStream_t s);
     void gen_windows(const GenGraph& g, const std::vector<GenWin>& w, std::vector<Act>& t, bool stream, const int* lens_or_null, const float* gdec,
                      int g_stride, float* o, cudaStream_t s);
     void g2_windows(const GenGraph& g, const std::vector<GenWin>& w, std::vector<H8>& t, bool stream, const float* gdec, int g_stride,
@@ -1112,16 +1121,17 @@ void bv2_engine::run_generator_g2(Act z, const int* lens, const float* gdec, int
     g2_windows(g, gen_stream_plan(g, z.T, 0, z.T), t, false, gdec, g_stride, o, s);
 }
 
-H8 bv2_engine::g2_h8(int B, int C, int T) {
-    H8 t; t.B = B; t.C = C; t.T = T; t.Tp = G2_PADL + T + G2_PADR;
-    t.p = reinterpret_cast<uint4*>(ws.alloc(H8::bytes(B, C, T) / 4)) + G2_PADL;
+// rows >= 0: storage for only that many rows (a bounded stream's tensor, H8::base); else the whole tensor
+H8 bv2_engine::g2_h8(int B, int C, int T, int rows) {
+    H8 t; t.B = B; t.C = C; t.T = T; t.Tp = G2_PADL + (rows >= 0 ? rows : T) + G2_PADR;
+    t.p = reinterpret_cast<uint4*>(ws.alloc(H8::bytes(B, C, t.Tp - G2_PADL - G2_PADR) / 4)) + G2_PADL;
     return t;
 }
 
 // z * y_mask as the raw f16 H8 tensor conv_pre reads (zero halos: every producer clears the halo rows of its own output)
 H8 bv2_engine::g2_input(Act z, const int* lens, cudaStream_t s) {
     H8 zh = g2_h8(z.B, z.C, z.T);
-    k_c4_to_h8<<<dim3(cdiv(z.T, 128), z.C / 8, z.B), 128, 0, s>>>(reinterpret_cast<const float4*>(z.p), zh.p, z.C, z.T, zh.Tp, lens);
+    k_c4_to_h8<<<dim3(cdiv(z.T, 128), z.C / 8, z.B), 128, 0, s>>>(reinterpret_cast<const float4*>(z.p), zh.p, z.C, z.T, zh.Tp, lens, 0, z.T, 0);
     BV2_CUDA(cudaGetLastError()); launches++;
     return zh;
 }
@@ -1145,11 +1155,28 @@ size_t bv2_engine::gen_stream_bytes(int B, int Fg) const {
     return n;
 }
 
-void bv2_engine::gen_stream_open(Act z, const int* lens, const float* gdec, int g_stride, float* o, cudaStream_t s) {
+// Workspace bytes of a stream's Generator tensors with chunks of at most max_chunk frames: a bounded stream's storage (independent of
+// Fg), else gen_stream_bytes
+size_t bv2_engine::stream_bytes(int B, int Fg, int max_chunk) const {
+    if (!stream_bounded(Fg, max_chunk)) return gen_stream_bytes(B, Fg);
+    const GenGraph g = gen_graph(cfg, max_chunk + 1);  // channels only: they do not depend on the length
+    const std::vector<int> cap = gen_stream_capacity(cfg, max_chunk);
+    size_t n = 0;
+    for (size_t i = 0; i + 1 < cap.size(); i++) n += (H8::bytes(B, gen_channels(g, (int)i), cap[i]) + 255) & ~(size_t)255;
+    return n;
+}
+
+void bv2_engine::gen_stream_open(Act z, const int* lens, const float* gdec, int g_stride, float* o, int max_chunk, cudaStream_t s) {
     gs.g = gen_graph(cfg, z.T);
     const size_t n = gs.g.tensor_len.size();
-    gs.t.clear(); gs.a.clear();
-    if (use_g2) {
+    gs.t.clear(); gs.a.clear(); gs.cap.clear();
+    gs.max_chunk = stream_bounded(z.T, max_chunk) ? max_chunk : 0;
+    if (gs.max_chunk) {
+        gs.cap = gen_stream_capacity(cfg, gs.max_chunk);
+        gs.t.assign(n, H8());
+        for (size_t i = 0; i + 1 < n; i++) gs.t[i] = g2_h8(z.B, gen_channels(gs.g, (int)i), gs.g.tensor_len[i], gs.cap[i]);
+        gs.z = z; gs.zlens = lens;
+    } else if (use_g2) {
         gs.t.assign(n, H8());
         gs.t[0] = g2_input(z, lens, s);
         for (size_t i = 1; i + 1 < n; i++) gs.t[i] = g2_h8(z.B, gen_channels(gs.g, (int)i), gs.g.tensor_len[i]);
@@ -1160,6 +1187,34 @@ void bv2_engine::gen_stream_open(Act z, const int* lens, const float* gdec, int 
     }
     gs.B = z.B; gs.Fg = z.T; gs.frontier = 0; gs.o = o; gs.gdec = gdec; gs.g_stride = g_stride; gs.lens = lens;
     gs.open = true;
+}
+
+// Before the windows of the chunk done -> target of a bounded stream: one slide launch for the tensors whose storage the chunk would
+// overrun (gen_stream_slides), then the conversion of the input rows the chunk reads.
+void bv2_engine::g2_stream_prepare(int done, int target, cudaStream_t s) {
+    const size_t n = gs.t.size();
+    std::vector<int> base(n);
+    for (size_t i = 0; i < n; i++) base[i] = gs.t[i].base;
+    const std::vector<GenSlide> sl = gen_stream_slides(gs.g, gs.Fg, gs.cap, base, done, target);
+    for (size_t k = 0; k < sl.size(); k += G2_SLIDE_MAX) {  // one launch at the default configuration (87 tensors)
+        G2SlideParams sp{};
+        int most = 0;
+        for (size_t j = k; j < sl.size() && sp.n < G2_SLIDE_MAX; j++) {
+            const H8& t = gs.t[sl[j].tensor];
+            sp.d[sp.n++] = G2SlideDesc{t.p, t.B * (t.C / 8), t.Tp, sl[j].src, sl[j].dst, sl[j].rows};
+            most = std::max(most, t.B * (t.C / 8) * sl[j].rows);
+        }
+        launch_pdl(k_g2_slide, dim3(std::min(32, cdiv(most, 256)), sp.n), dim3(256), 0, s, sp);
+        launches++;
+    }
+    for (size_t i = 0; i < n; i++) gs.t[i].base = base[i];
+    const int a = gen_needs(gs.g, gs.Fg, done).tensor[0], b = gen_needs(gs.g, gs.Fg, target).tensor[0];
+    if (b > a) {
+        const Act& z = gs.z;
+        k_c4_to_h8<<<dim3(cdiv(b - a, 128), z.C / 8, z.B), 128, 0, s>>>(reinterpret_cast<const float4*>(z.p), gs.t[0].p, z.C, z.T, gs.t[0].Tp, gs.zlens,
+                                                                      a, b, gs.t[0].base);
+        BV2_CUDA(cudaGetLastError()); launches++;
+    }
 }
 
 // Runs every Generator layer over its window of w (GenGraph launch order; empty windows launch nothing) on the H8 tensors t, one per
@@ -1231,8 +1286,13 @@ void bv2_engine::g2_windows(const GenGraph& g, const std::vector<GenWin>& w, std
     BV2_CHECK(x.C == 16, "conv_post kernel instantiated for 16 input channels");
     const GenWin& wp = w[li];
     if (wp.t_end > wp.t_begin) {
-        launch_pdl(k_conv_post_tanh_h8<16, 7>, dim3(cdiv(wp.t_end - wp.t_begin, 512), B), dim3(256), 0, s, (const uint4*)x.p, x.Tp, conv_post_h, o,
-                   lp.L_out, wp.t_begin, wp.t_end);
+        BV2_CHECK((x.base == 0 || wp.t_begin - 3 >= x.base) && std::min(wp.t_end + 3, x.T + G2_PADR) <= x.lim(), "conv_post input rows not resident");
+        const dim3 grid(cdiv(wp.t_end - wp.t_begin, 512), B);
+        if (x.base == 0 && x.Tp == G2_PADL + x.T + G2_PADR)
+            launch_pdl(k_conv_post_tanh_h8<16, 7>, grid, dim3(256), 0, s, (const uint4*)x.p, x.Tp, conv_post_h, o, lp.L_out, wp.t_begin, wp.t_end);
+        else  // a bounded stream's resident rows
+            launch_pdl(k_conv_post_tanh_h8_resident<16, 7>, grid, dim3(256), 0, s, (const uint4*)x.p, x.Tp, x.base, conv_post_h, o, lp.L_out, wp.t_begin,
+                       wp.t_end);
         launches++;
     }
 }
@@ -1252,14 +1312,26 @@ void bv2_engine::g2_windows(const GenGraph& g, const std::vector<GenWin>& w, std
     catch (const std::exception& ex) { (e)->err = ex.what(); return BV2_ERR_INTERNAL; } \
     return BV2_OK;
 
-static size_t ws_bytes_for(const bv2_config& c, int B, int T, int F) {
-    // generous upper bounds; every buffer is bump-allocated per call
+// Workspace of a call, in two parts (generous upper bounds; every buffer is bump-allocated per call): the encoder, durations and flow,
+// and the one-shot Generator's stage temporaries.  A Generator stream needs the first part plus its own tensors (stream_bytes).
+static size_t ws_enc_flow_bytes(const bv2_config& c, int B, int T, int F) {
     size_t tok = (size_t)B * T, frm = (size_t)B * std::max(F, 1);
     size_t enc = tok * (3 * c.bert_dim + 16 * c.hidden_channels + c.filter_channels + 2 * c.dp_filter + 64) * 4;
     size_t flow = frm * (12 * c.hidden_channels + c.filter_channels + 4 * c.inter_channels) * 4 +
                   (size_t)B * c.n_heads * ((size_t)F + 128) * ((size_t)F + 96) * 4 + (1u << 20);  // attention S/P + V^T
-    size_t gen = frm * ((size_t)c.upsample_initial_channel + 8192ull * (5 + 10) + 4096) * 4;  // 5 stage outputs + 10 temporaries (3 resblock chains)
-    return enc + flow + gen + (64u << 20);
+    return enc + flow + (64u << 20);
+}
+static size_t ws_gen_bytes(const bv2_config& c, int B, int F) {
+    const size_t frm = (size_t)B * std::max(F, 1);
+    return frm * ((size_t)c.upsample_initial_channel + 8192ull * (5 + 10) + 4096) * 4;  // 5 stage outputs + 10 temporaries (3 resblock chains)
+}
+static size_t ws_bytes_for(const bv2_config& c, int B, int T, int F) { return ws_enc_flow_bytes(c, B, T, F) + ws_gen_bytes(c, B, F); }
+
+// Workspace a stream over F frames (Fg of them through the Generator) ensures.  max_chunk <= 0: the unbounded stream, which has always
+// reserved the one-shot Generator's part as well; a cap: the encoder/flow part plus the stream's own tensors.
+static size_t ws_stream_bytes(const bv2_engine* e, int B, int T, int F, int Fg, int max_chunk) {
+    if (max_chunk <= 0) return ws_bytes_for(e->cfg, B, T, F) + e->gen_stream_bytes(B, Fg);
+    return ws_enc_flow_bytes(e->cfg, B, T, F) + e->stream_bytes(B, Fg, max_chunk);
 }
 
 static size_t persist_bytes_for(const bv2_config& c, int B, int T, int gproj_n) {
@@ -1455,7 +1527,8 @@ int bv2_infer_begin(bv2_engine* e, int B, int T, const int64_t* x, const int64_t
 
 // open_stream: stop after the flow and open a Generator stream over o instead of running the Generator (bv2_infer_finish_stream)
 static int infer_finish_impl(bv2_engine* e, const float* noise_z, int64_t noise_ld, float noise_scale, int32_t max_len, float* o, int16_t* o16,
-                             float* attn, float* y_mask, float* z_out, float* z_p, float* m_p, float* logs_p, void* stream, bool open_stream = false) {
+                             float* attn, float* y_mask, float* z_out, float* z_p, float* m_p, float* logs_p, void* stream, bool open_stream = false,
+                             int max_chunk = 0) {
     BV2_API_BEGIN(e)
     auto& st = e->st;
     BV2_CHECK(st.active, "infer_finish without infer_begin");
@@ -1464,7 +1537,9 @@ static int infer_finish_impl(bv2_engine* e, const float* noise_z, int64_t noise_
     const bv2_config& c = e->cfg;
     const int B = st.B, T = st.T, F = st.F, I = c.inter_channels;
     const int Fg = (max_len > 0 && max_len < F) ? max_len : F;
-    e->ws.ensure(ws_bytes_for(c, B, T, F) + (open_stream ? e->gen_stream_bytes(B, Fg) : 0));
+    if (open_stream && !e->use_g2 && max_chunk >= 1 && max_chunk < Fg)
+        throw Error(BV2_ERR_ARG, "a chunk cap below the frame count needs the FP16 Generator (precision fp16 or fp16g)");
+    e->ws.ensure(open_stream ? ws_stream_bytes(e, B, T, F, Fg, max_chunk) : ws_bytes_for(c, B, T, F));
     e->ws_reset();
     float* m_tmp = m_p ? m_p : e->ws.alloc((size_t)B * I * F);
     float* l_tmp = logs_p ? logs_p : e->ws.alloc((size_t)B * I * F);
@@ -1496,7 +1571,7 @@ static int infer_finish_impl(bv2_engine* e, const float* noise_z, int64_t noise_
         BV2_CUDA(cudaMemcpy2DAsync(zg.p, (size_t)Fg * 16, z.p, (size_t)F * 16, (size_t)Fg * 16, (size_t)B * I / 4, cudaMemcpyDeviceToDevice, s));
     }
     if (open_stream) {
-        e->gen_stream_open(zg, st.ylen32, st.gproj + e->goff_dec, e->gproj_n, o, s);
+        e->gen_stream_open(zg, st.ylen32, st.gproj + e->goff_dec, e->gproj_n, o, max_chunk, s);
         st.active = false; st.finished = true;
         return BV2_OK;
     }
@@ -1530,10 +1605,16 @@ int bv2_infer_finish_pcm16(bv2_engine* e, const float* noise_z, int64_t noise_ld
     return infer_finish_impl(e, noise_z, noise_ld, noise_scale, max_len, nullptr, o16, attn, y_mask, z_out, z_p, m_p, logs_p, stream);
 }
 
+int bv2_infer_finish_stream_bounded(bv2_engine* e, const float* noise_z, int64_t noise_ld, float noise_scale, int32_t max_len, int32_t max_chunk_frames,
+                                    float* o, float* attn, float* y_mask, float* z_out, float* z_p, float* m_p, float* logs_p, void* stream) {
+    if (!o) return BV2_ERR_ARG;
+    return infer_finish_impl(e, noise_z, noise_ld, noise_scale, max_len, o, nullptr, attn, y_mask, z_out, z_p, m_p, logs_p, stream, true,
+                             std::max<int32_t>(max_chunk_frames, 0));
+}
+
 int bv2_infer_finish_stream(bv2_engine* e, const float* noise_z, int64_t noise_ld, float noise_scale, int32_t max_len, float* o,
                             float* attn, float* y_mask, float* z_out, float* z_p, float* m_p, float* logs_p, void* stream) {
-    if (!o) return BV2_ERR_ARG;
-    return infer_finish_impl(e, noise_z, noise_ld, noise_scale, max_len, o, nullptr, attn, y_mask, z_out, z_p, m_p, logs_p, stream, true);
+    return bv2_infer_finish_stream_bounded(e, noise_z, noise_ld, noise_scale, max_len, 0, o, attn, y_mask, z_out, z_p, m_p, logs_p, stream);
 }
 
 int bv2_stream_advance(bv2_engine* e, int32_t frames, void* stream, int64_t* samples_ready) {
@@ -1541,9 +1622,12 @@ int bv2_stream_advance(bv2_engine* e, int32_t frames, void* stream, int64_t* sam
     auto& gs = e->gs;
     if (!gs.open) throw Error(BV2_ERR_STATE, "stream_advance without an open stream");
     if (frames <= gs.frontier) throw Error(BV2_ERR_STATE, "stream_advance: frames must exceed the frames already final");
+    if (gs.max_chunk && (int64_t)frames - gs.frontier > gs.max_chunk)
+        throw Error(BV2_ERR_ARG, "stream_advance: the chunk exceeds the stream's max_chunk_frames");
     const int f = std::min<int>(frames, gs.Fg);
     const std::vector<GenWin> w = gen_stream_plan(gs.g, gs.Fg, gs.frontier, f);
     cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (gs.max_chunk) e->g2_stream_prepare(gs.frontier, f, s);
     if (e->use_g2) e->g2_windows(gs.g, w, gs.t, true, gs.gdec, gs.g_stride, gs.o, s);
     else e->gen_windows(gs.g, w, gs.a, true, gs.lens, gs.gdec, gs.g_stride, gs.o, s);
     gs.frontier = f;
@@ -1574,16 +1658,45 @@ int bv2_wave_to_pcm16(bv2_engine* e, int B, int64_t L, const float* wave, const 
     BV2_API_END(e)
 }
 
-int bv2_reserve(bv2_engine* e, int B, int T, int F_cap) {
+// Workspace that covers every call within (B, T, F_cap) and, with with_stream, every stream with chunks of at most max_chunk frames
+// (max_chunk <= 0: unbounded streams).  A stream over Fg <= max_chunk frames is unbounded, and its tensors are no larger than the
+// bounded storage for max_chunk; the workspace needs grow with F otherwise.
+static size_t reserve_bytes(const bv2_engine* e, int B, int T, int F_cap, bool with_stream, int max_chunk) {
+    size_t need = ws_bytes_for(e->cfg, B, T, F_cap);
+    if (!with_stream) return need;
+    need = std::max(need, ws_stream_bytes(e, B, T, F_cap, F_cap, max_chunk));
+    if (max_chunk >= 1) need = std::max(need, ws_enc_flow_bytes(e->cfg, B, T, F_cap) + e->stream_bytes(B, std::min(F_cap, max_chunk), max_chunk));
+    return need;
+}
+
+static int reserve_impl(bv2_engine* e, int B, int T, int F_cap, bool with_stream, int max_chunk) {
     BV2_API_BEGIN(e)
     BV2_CHECK(e->finalized && B >= 1 && T >= 1 && F_cap >= 1, "reserve args");
     const bv2_config& c = e->cfg;
-    const size_t need = ws_bytes_for(c, B, T, F_cap);
+    if (with_stream && !e->use_g2 && max_chunk >= 1 && max_chunk < F_cap)
+        throw Error(BV2_ERR_ARG, "a chunk cap below the frame count needs the FP16 Generator (precision fp16 or fp16g)");
+    const size_t need = reserve_bytes(e, B, T, F_cap, with_stream, max_chunk);
     const size_t pneed = persist_bytes_for(c, B, T, e->gproj_n);
     if (need > e->ws.cap() || pneed > e->persist.cap()) e->gs.open = false;  // regrowing an arena frees what an open stream reads
     e->ws.ensure(need);
     e->persist.ensure(pneed);
     BV2_API_END(e)
+}
+
+int bv2_reserve(bv2_engine* e, int B, int T, int F_cap) { return reserve_impl(e, B, T, F_cap, false, 0); }
+
+int bv2_reserve_stream(bv2_engine* e, int B, int T, int F_cap, int32_t max_chunk_frames) {
+    return reserve_impl(e, B, T, F_cap, true, std::max<int32_t>(max_chunk_frames, 0));
+}
+
+int64_t bv2_stream_bytes(const bv2_engine* e, int B, int32_t Fg, int32_t max_chunk_frames) {
+    if (!e || !e->finalized || B < 1 || Fg < 1) return BV2_ERR_ARG;
+    const int32_t cap = std::max<int32_t>(max_chunk_frames, 0);
+    if (((int64_t)std::max(Fg, cap) + 1024) * e->hop > INT32_MAX) return BV2_ERR_ARG;  // rows of the waveform must fit an int
+    if (!e->use_g2 && cap >= 1 && cap < Fg) return BV2_ERR_ARG;
+    try {
+        return (int64_t)e->stream_bytes(B, Fg, cap);
+    } catch (const std::exception&) { return BV2_ERR_INTERNAL; }
 }
 
 int bv2_text_encoder(bv2_engine* e, int B, int T, const int64_t* x, const int64_t* x_lengths, const int64_t* sid,

@@ -68,9 +68,14 @@ inline GenGraph gen_graph(const bv2_config& c, int Fg) {
     return g;
 }
 
-// End of the output range every layer must have computed for `frontier` (clamped to [0, Fg]) frames of final audio.
-inline std::vector<int> gen_need(const GenGraph& g, int Fg, int frontier) {
-    std::vector<int> tneed(g.tensor_len.size(), 0), lneed(g.layers.size(), 0);
+// End of the output range every layer (layer) and every tensor (tensor: the rows its consumers read) must have computed for
+// `frontier` (clamped to [0, Fg]) frames of final audio.
+struct GenNeed { std::vector<int> layer, tensor; };
+inline GenNeed gen_needs(const GenGraph& g, int Fg, int frontier) {
+    GenNeed r;
+    std::vector<int>& tneed = r.tensor;
+    std::vector<int>& lneed = r.layer;
+    tneed.assign(g.tensor_len.size(), 0); lneed.assign(g.layers.size(), 0);
     tneed[g.layers.back().out] = std::min(std::max(frontier, 0), Fg) * g.hop;
     for (int li = (int)g.layers.size() - 1; li >= 0; li--) {  // consumers come after their producers in launch order
         const GenLayer& l = g.layers[li];
@@ -78,11 +83,13 @@ inline std::vector<int> gen_need(const GenGraph& g, int Fg, int frontier) {
         if (n <= 0) continue;
         if (l.u > 1) n = std::min(l.L_out, (n + l.u - 1) / l.u * l.u);
         lneed[li] = n;
+        tneed[l.out] = n;
         tneed[l.in] = std::max(tneed[l.in], std::min(l.L_in, n / l.u + l.reach));
         if (l.res >= 0) tneed[l.res] = std::max(tneed[l.res], n);
     }
-    return lneed;
+    return r;
 }
+inline std::vector<int> gen_need(const GenGraph& g, int Fg, int frontier) { return gen_needs(g, Fg, frontier).layer; }
 
 // The windows of one chunk: everything that makes frames [done, target) of audio final, given that frames [0, done) already are.
 inline std::vector<GenWin> gen_stream_plan(const GenGraph& g, int Fg, int done, int target) {
@@ -90,6 +97,67 @@ inline std::vector<GenWin> gen_stream_plan(const GenGraph& g, int Fg, int done, 
     std::vector<GenWin> w(g.layers.size());
     for (size_t i = 0; i < w.size(); i++) { w[i].t_begin = a[i]; w[i].t_end = std::max(a[i], b[i]); }
     return w;
+}
+
+// ---- bounded streams: every tensor but the waveform keeps only a range of its rows resident.
+// Logical row t of a tensor lives at physical row t - base of a storage of `capacity` rows (plus the zero halos).  After the frontier
+// reaches `done`, no future window reads a row below resident_begin: a conv consumer with done pointer d reads from d / u - reach, a
+// residual read from d.  The rows [resident_begin(done), need(done)) are final and still read; the rows below are dead.
+inline std::vector<int> gen_resident_begin(const GenGraph& g, int Fg, int done) {
+    const std::vector<int> d = gen_need(g, Fg, done);
+    std::vector<int> lo(g.tensor_len);  // a tensor nobody reads any more keeps nothing
+    for (size_t li = 0; li < g.layers.size(); li++) {
+        const GenLayer& l = g.layers[li];
+        lo[l.in] = std::min(lo[l.in], d[li] / l.u - l.reach);
+        if (l.res >= 0) lo[l.res] = std::min(lo[l.res], d[li]);
+    }
+    for (size_t i = 0; i < lo.size(); i++) lo[i] = std::max(0, std::min(lo[i], g.tensor_len[i]));
+    return lo;
+}
+
+// Rows of storage each tensor needs for any chunk schedule whose chunks are at most max_chunk_frames >= 1 frames, for any Fg.  A chunk
+// done -> target touches the rows [resident_begin(done), need(target)) of a tensor; away from the ends of the utterance both bounds
+// are affine in the frame count (every rate is a whole multiple of the ConvTranspose strides), so that span is rows_per_frame *
+// max_chunk_frames + keep, with keep = need(done) - resident_begin(done) the rows a slide carries over.  The capacity is span + keep:
+// a slide happens only when the span no longer fits behind the current base, which then drops more than `keep` rows, so a slide's
+// source never overlaps its destination.  Near the ends the clamps to [0, L] only shrink both terms.  The one exception is the first
+// chunk: at frontier 0 every done pointer is 0 rather than affine, so it touches need(max_chunk_frames) rows from row 0.  The
+// waveform (the caller's buffer) gets 0.
+inline std::vector<int> gen_stream_capacity(const bv2_config& c, int max_chunk_frames) {
+    BV2_CHECK(max_chunk_frames >= 1, "gen_stream_capacity: cap >= 1");
+    for (int d0 = 64;; d0 *= 2) {  // a frontier far enough from both ends that no clamp applies
+        const int Fv = 2 * d0 + max_chunk_frames;
+        const GenGraph g = gen_graph(c, Fv);
+        const std::vector<int> lo = gen_resident_begin(g, Fv, d0), n0 = gen_needs(g, Fv, d0).tensor, n1 = gen_needs(g, Fv, d0 + max_chunk_frames).tensor;
+        const size_t nt = g.tensor_len.size();
+        bool interior = true;
+        for (size_t i = 0; i + 1 < nt; i++) interior = interior && lo[i] > 0 && n1[i] < g.tensor_len[i];
+        if (!interior) { BV2_CHECK(d0 < (1 << 20), "gen_stream_capacity"); continue; }
+        // the first chunk starts from nothing (every done pointer is 0, so it runs the whole lead of the wavefront) and never slides
+        const std::vector<int> first = gen_needs(g, Fv, max_chunk_frames).tensor;
+        std::vector<int> cap(nt, 0);
+        for (size_t i = 0; i + 1 < nt; i++) cap[i] = std::max((n1[i] - lo[i]) + (n0[i] - lo[i]), first[i]);
+        return cap;
+    }
+}
+
+// One slide: rows [src, src + rows) of every row block of tensor `tensor` move to [dst, dst + rows) (physical rows, dst < src).
+struct GenSlide { int tensor, src, dst, rows; };
+
+// Slides that let the chunk done -> target fit in the capacities cap (gen_stream_capacity), given the current bases (updated in place;
+// the waveform, the last tensor, is never bounded).  A tensor slides only when the chunk's rows would run past its storage; its base
+// then becomes resident_begin(done) and the final rows it still reads, [resident_begin(done), need(done)), move to the front.
+inline std::vector<GenSlide> gen_stream_slides(const GenGraph& g, int Fg, const std::vector<int>& cap, std::vector<int>& base, int done, int target) {
+    std::vector<GenSlide> s;
+    const std::vector<int> lo = gen_resident_begin(g, Fg, done), n0 = gen_needs(g, Fg, done).tensor, n1 = gen_needs(g, Fg, target).tensor;
+    for (size_t i = 0; i + 1 < g.tensor_len.size(); i++) {
+        if (n1[i] - base[i] <= cap[i]) continue;
+        const int keep = std::max(0, n0[i] - lo[i]), drop = lo[i] - base[i];
+        BV2_CHECK(n1[i] - lo[i] <= cap[i] && drop >= keep, "bounded stream: a chunk exceeds the capacity it was planned for");
+        if (keep > 0) s.push_back(GenSlide{(int)i, drop, 0, keep});
+        base[i] = lo[i];
+    }
+    return s;
 }
 
 }  // namespace bv2

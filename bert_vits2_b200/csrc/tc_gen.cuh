@@ -32,10 +32,16 @@ namespace bv2 {
 
 constexpr int G2_PADL = 32, G2_PADR = 32;  // zero halo rows before t = 0 / after t = T-1 (max conv padding: (11-1)/2*5 = 25)
 
-// 16-bit Generator activation; p points at row t = 0 of (b = 0, channel group 0); rows [-G2_PADL, T + G2_PADR) are allocated.
+// 16-bit Generator activation; p points at physical row 0 of (b = 0, channel group 0); physical rows [-G2_PADL, Tp - G2_PADL) are
+// allocated.  Logical row t (t in [-G2_PADL, T + G2_PADR)) lives at physical row t - base.  A whole tensor has base 0 and
+// Tp = G2_PADL + T + G2_PADR; a tensor of a bounded stream (gen_stream.cuh) holds only the rows [base, base + Tp - G2_PADL).
 struct H8 {
     uint4* p = nullptr;
-    int B = 0, C = 0, T = 0, Tp = 0;
+    int B = 0, C = 0, T = 0, Tp = 0, base = 0;
+    int lim() const { return base + Tp - G2_PADL; }  // logical end of the storage
+    // address of logical row 0 of (b = 0, channel group 0): row t of block k is row0()[k * Tp + t] for resident t.  With base > 0 this
+    // points before the allocation, so it is computed as an integer address and only ever offset back into the storage.
+    uint4* row0() const { return reinterpret_cast<uint4*>(reinterpret_cast<uintptr_t>(p) - (uintptr_t)base * sizeof(uint4)); }
     static size_t bytes(int B, int C, int T) { return (size_t)B * (C / 8) * (size_t)(G2_PADL + T + G2_PADR) * 16; }
 };
 
@@ -47,6 +53,7 @@ struct G2Params {
     uint32_t a_stage_bytes, w_stage_bytes, acc_cols;  // acc_cols: columns of the accumulator image
     int residual, accumulate, ups_u, ups_cout;
     float out_scale;
+    int x_lim;  // end of the input rows that may be read: the halo's end T + G2_PADR, or the storage's end if that comes first
 };
 
 namespace tc {
@@ -152,7 +159,7 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
         for (int s = 0; s < steps; s++) {
             const int g = s / NCH, c = s - g * NCH, sa = s % NAS;
             const int row0 = t0 + g * MG * 128 - p.pad;
-            const int nrows = max(0, min(R, p.T + G2_PADR - row0));  // never read past the tensor's halo; rows beyond (and rows past a window's end) feed discarded outputs only
+            const int nrows = max(0, min(R, p.x_lim - row0));  // never read past the tensor's halo or storage; rows beyond (and rows past a window's end) feed discarded outputs only
             if (lane == 0) {
                 mbar_wait(BAR(B_AEMPTY + sa), ((s / NAS) & 1) ^ 1);
                 mbar_expect_tx(BAR(B_AFULL + sa), (uint32_t)nrows * 16u * (uint32_t)ncg);
@@ -321,19 +328,21 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
     __syncthreads();
 }
 
-// fp32 c4 [B][C/4][T][4] (rows t >= lens[b] read as zero) -> raw f16 H8 (no activation): the Generator's input z * y_mask
-__global__ void __launch_bounds__(128) k_c4_to_h8(const float4* __restrict__ x, uint4* __restrict__ y, int C, int T, int Tp, const int* __restrict__ lens) {
-    const int t = blockIdx.x * blockDim.x + threadIdx.x, g = blockIdx.y, b = blockIdx.z;
-    // zero halo of the output (conv_pre's padding): first / last block of each channel-group run
-    if (blockIdx.x == 0 && threadIdx.x < G2_PADL) y[((size_t)b * (C / 8) + g) * Tp + (int)threadIdx.x - G2_PADL] = make_uint4(0u, 0u, 0u, 0u);
-    if (blockIdx.x == gridDim.x - 1 && threadIdx.x < G2_PADR) y[((size_t)b * (C / 8) + g) * Tp + T + threadIdx.x] = make_uint4(0u, 0u, 0u, 0u);
-    if (t >= T) return;
+// fp32 c4 [B][C/4][T][4] (rows t >= lens[b] read as zero) -> raw f16 H8 (no activation): the Generator's input z * y_mask, rows
+// [t_begin, t_end) of it, into an H8 whose physical row 0 is logical row y_base
+__global__ void __launch_bounds__(128) k_c4_to_h8(const float4* __restrict__ x, uint4* __restrict__ y, int C, int T, int Tp, const int* __restrict__ lens,
+                                                  int t_begin, int t_end, int y_base) {
+    const int t = t_begin + blockIdx.x * blockDim.x + threadIdx.x, g = blockIdx.y, b = blockIdx.z;
+    // zero halo of the output (conv_pre's padding): first / last block of each channel-group run, when the window reaches that end
+    if (blockIdx.x == 0 && t_begin == 0 && threadIdx.x < G2_PADL) y[((size_t)b * (C / 8) + g) * Tp + (int)threadIdx.x - G2_PADL] = make_uint4(0u, 0u, 0u, 0u);
+    if (blockIdx.x == gridDim.x - 1 && t_end == T && threadIdx.x < G2_PADR) y[((size_t)b * (C / 8) + g) * Tp + (T - y_base) + threadIdx.x] = make_uint4(0u, 0u, 0u, 0u);
+    if (t >= t_end) return;
     const bool in = !lens || t < lens[b];
     float4 a = make_float4(0.f, 0.f, 0.f, 0.f), c = a;
     if (in) { a = x[((size_t)b * (C / 4) + 2 * g) * T + t]; c = x[((size_t)b * (C / 4) + 2 * g + 1) * T + t]; }
     uint4 o;
     o.x = tc::pack_h2(a.x, a.y); o.y = tc::pack_h2(a.z, a.w); o.z = tc::pack_h2(c.x, c.y); o.w = tc::pack_h2(c.z, c.w);
-    y[((size_t)b * (C / 8) + g) * Tp + t] = o;
+    y[((size_t)b * (C / 8) + g) * Tp + (t - y_base)] = o;
 }
 
 // conv_post (C -> 1, K taps, no bias) + tanh on an H8 input (reference models.py:553-555: F.leaky_relu default slope 0.01,
@@ -343,18 +352,19 @@ __global__ void __launch_bounds__(128) k_c4_to_h8(const float4* __restrict__ x, 
 // stages TB + K - 1 rows ONCE as activated fp32 in shared memory (coalesced 16-byte loads, conflict-free stores), the weights ride in the
 // kernel parameters (constant bank: FFMA takes them as an operand), and a thread's inner loop is one conflict-free LDS + one FFMA per tap.
 template <int C, int K> struct PostW { float w[C * K]; };  // [C][K]
-// Outputs [t_begin, t_end) of the T samples are stored; staged rows past t_end feed discarded outputs only.
+// Outputs [t_begin, t_end) of the T samples are stored; staged rows past t_end feed discarded outputs only.  x holds the logical rows
+// [x_base, row_end) (H8::base); rows from row_end on are read as zero.
 template <int C, int K>
-__global__ void __launch_bounds__(256) k_conv_post_tanh_h8(const uint4* __restrict__ x, int Tp, const __grid_constant__ PostW<C, K> pw, float* __restrict__ y, int T,
-                                                           int t_begin, int t_end) {
+__device__ __forceinline__ void conv_post_tanh_h8(const uint4* __restrict__ x, int Tp, int x_base, int row_end, const PostW<C, K>& pw,
+                                                  float* __restrict__ y, int T, int t_begin, int t_end) {
     constexpr int TB = 512, RW = TB + K - 1, LD = RW + 2;  // outputs per block, staged rows, row stride of the staged tile
     __shared__ float sx[C][LD];
     asm volatile("griddepcontrol.wait;" ::: "memory");
     const int t0 = t_begin + blockIdx.x * TB, b = blockIdx.y;
     for (int i = threadIdx.x; i < (C / 8) * RW; i += blockDim.x) {
-        const int g = i / RW, r = i - g * RW, row = t0 - K / 2 + r;  // row >= -K/2 >= -G2_PADL; rows >= T + G2_PADR lie outside the allocation
+        const int g = i / RW, r = i - g * RW, row = t0 - K / 2 + r;  // row >= -K/2 >= -G2_PADL
         float f[8];
-        if (row < T + G2_PADR) tc::unpack8(x[((size_t)b * (C / 8) + g) * Tp + row], f);
+        if (row < row_end) tc::unpack8(x[((size_t)b * (C / 8) + g) * Tp + (row - x_base)], f);
         else {
 #pragma unroll
             for (int k = 0; k < 8; k++) f[k] = 0.f;
@@ -376,6 +386,35 @@ __global__ void __launch_bounds__(256) k_conv_post_tanh_h8(const uint4* __restri
             }
         }
         if (t < t_end) y[(size_t)b * T + t] = tanhf(acc);
+    }
+}
+// A whole H8 input (rows [-G2_PADL, T + G2_PADR) allocated)
+template <int C, int K>
+__global__ void __launch_bounds__(256) k_conv_post_tanh_h8(const uint4* __restrict__ x, int Tp, const __grid_constant__ PostW<C, K> pw, float* __restrict__ y, int T,
+                                                           int t_begin, int t_end) {
+    conv_post_tanh_h8<C, K>(x, Tp, 0, T + G2_PADR, pw, y, T, t_begin, t_end);
+}
+// The input of a bounded stream (H8 with base x_base): rows past the storage's end read as zero like the halo past T + G2_PADR
+template <int C, int K>
+__global__ void __launch_bounds__(256) k_conv_post_tanh_h8_resident(const uint4* __restrict__ x, int Tp, int x_base, const __grid_constant__ PostW<C, K> pw,
+                                                                    float* __restrict__ y, int T, int t_begin, int t_end) {
+    conv_post_tanh_h8<C, K>(x, Tp, x_base, min(T + G2_PADR, x_base + Tp - G2_PADL), pw, y, T, t_begin, t_end);
+}
+
+// Slide of a bounded stream (gen_stream_slides): for each descriptor, rows [src, src + rows) of every one of its `blocks` row blocks
+// (B x C/8, row stride Tp) move to [dst, dst + rows).  Source and destination never overlap (dst + rows <= src), so the copy has no
+// order.  16-byte vectors; blockIdx.y picks the descriptor.
+struct G2SlideDesc { uint4* p; int blocks, Tp, src, dst, rows; };  // p: physical row 0 of row block 0 (H8::p)
+constexpr int G2_SLIDE_MAX = 120;  // descriptors per launch: the parameter block stays below 4 KB
+struct G2SlideParams { int n; G2SlideDesc d[G2_SLIDE_MAX]; };
+__global__ void __launch_bounds__(256) k_g2_slide(const __grid_constant__ G2SlideParams sp) {
+    asm volatile("griddepcontrol.wait;" ::: "memory");  // the rows were written by the kernels before this one
+    const G2SlideDesc& d = sp.d[blockIdx.y];
+    const long long n = (long long)d.blocks * d.rows;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const int blk = (int)(i / d.rows), r = (int)(i - (long long)blk * d.rows);
+        uint4* row0 = d.p + (size_t)blk * d.Tp;
+        row0[d.dst + r] = row0[d.src + r];
     }
 }
 
@@ -414,9 +453,14 @@ inline G2Plan g2_conv_plan(const TcConvW& w, const float* bias, const H8& x, con
     BV2_CHECK(w.w && w.f16 && bias && x.B == y.B && y.T == x.T * u && x.C == w.Cin && (w.ups_u ? y.C == w.ups_cout : y.C == w.Cout), "g2_conv shapes");
     BV2_CHECK(w.nt <= 128 && (w.KC == 16 || w.KC == 32) && x.C % 8 == 0 && y.C % 8 == 0, "g2_conv tiling (K chunk of 16 or 32 channels)");
     p = G2Params{};
-    p.x = x.p; p.y = y.p; p.w = w.w; p.bias = bias; p.bias_b = e.bias_b; p.bias_b_stride = e.bias_b_stride;
+    // x, y and res are addressed by logical row: the pointers are H8::row0(), which only resident rows are read or written through
+    p.x = x.row0(); p.y = y.row0(); p.w = w.w; p.bias = bias; p.bias_b = e.bias_b; p.bias_b_stride = e.bias_b_stride;
     p.x_cg = x.C / 8; p.x_Tp = x.Tp; p.y_cg = y.C / 8; p.y_Tp = y.Tp;
-    if (e.res) { BV2_CHECK(!w.ups_u && e.res->C == y.C && e.res->T == y.T && e.res->B == y.B, "g2_conv residual"); p.res = e.res->p; p.res_cg = e.res->C / 8; p.res_Tp = e.res->Tp; p.residual = 1; }
+    p.x_lim = std::min(x.T + G2_PADR, x.lim());
+    if (e.res) {
+        BV2_CHECK(!w.ups_u && e.res->C == y.C && e.res->T == y.T && e.res->B == y.B, "g2_conv residual");
+        p.res = e.res->row0(); p.res_cg = e.res->C / 8; p.res_Tp = e.res->Tp; p.residual = 1;
+    }
     p.accumulate = e.accumulate; p.out_scale = e.out_scale; p.ups_u = w.ups_u; p.ups_cout = w.ups_cout;
     if (w.ups_u) BV2_CHECK(w.ups_cout % 8 == 0 && !e.accumulate, "g2_conv ups");
     p.T = x.T; p.K = w.K; p.dil = e.dil; p.pad = (w.K - 1) / 2 * e.dil;
@@ -425,6 +469,10 @@ inline G2Plan g2_conv_plan(const TcConvW& w, const float* bias, const H8& x, con
     const int t_end = e.t_end < 0 ? y.T : e.t_end;
     BV2_CHECK(0 <= e.t_begin && e.t_begin < t_end && t_end <= y.T && e.t_begin % u == 0 && t_end % u == 0, "g2_conv output window");
     p.t_begin = e.t_begin / u; p.t_end = t_end / u;
+    // every row the window reads or writes is resident (a whole tensor, base 0, always passes)
+    BV2_CHECK((x.base == 0 || p.t_begin - p.pad >= x.base) && std::min(p.t_end + p.pad, x.T + G2_PADR) <= x.lim(), "g2_conv input rows not resident");
+    BV2_CHECK((y.base == 0 || e.t_begin >= y.base) && (t_end < y.T ? t_end : y.T + G2_PADR) <= y.lim(), "g2_conv output rows not resident");
+    if (e.res) BV2_CHECK(e.t_begin >= e.res->base && t_end <= e.res->lim(), "g2_conv residual rows not resident");
     const int ntiles = w.Cout / w.nt, halo = (w.K - 1) * e.dil;
     p.w_stage_bytes = (uint32_t)(w.KC * w.nt * 2);
     // the accumulator image of a CTA holds at most 128 columns of 128 rows (66 KB of shared memory).  The time tiling follows the window;

@@ -50,6 +50,11 @@ def _ptr(t: Optional[torch.Tensor]):
     return None if t is None else C.c_void_p(t.data_ptr())
 
 
+def _cap(max_chunk_frames: Optional[int]) -> int:
+    """max_chunk_frames as the C ABI takes it: 0 = unbounded"""
+    return 0 if max_chunk_frames is None else max(0, int(max_chunk_frames))
+
+
 class Engine:
     """An engine on one CUDA device; it serves one request at a time (sibling() gives another over the same weights).  precision: 'fp32' (SIMT FMA everywhere), 'tf32' (wgmma implicit-GEMM convs with TF32
     operands) or 'fp16' (wgmma with FP16 operands -- same 11-bit significand as TF32, twice the tensor rate, half the
@@ -142,6 +147,20 @@ class Engine:
         """Size the workspace up front for batches up to (B, T tokens, F_cap frames): no allocation / device sync afterwards."""
         self._check(self.lib.bv2_reserve(self._h, int(B), int(T), int(F_cap)))
 
+    def reserve_stream(self, B: int, T: int, F_cap: int, max_chunk_frames: Optional[int]):
+        """reserve() plus room for one stream with chunks of at most max_chunk_frames (None: an unbounded stream) over up to F_cap
+        frames: afterwards no call and no such stream within those bounds grows the workspace."""
+        self._check(self.lib.bv2_reserve_stream(self._h, int(B), int(T), int(F_cap), _cap(max_chunk_frames)))
+
+    def stream_bytes(self, B: int, Fg: int, max_chunk_frames: Optional[int]) -> int:
+        """Workspace bytes of the Generator tensors of a stream over Fg frames with chunks of at most max_chunk_frames (computed, not
+        measured): for a cap below Fg the bounded storage, which does not depend on Fg; else what an unbounded stream allocates."""
+        n = int(self.lib.bv2_stream_bytes(self._h, int(B), int(Fg), _cap(max_chunk_frames)))
+        if n < 0:
+            raise ValueError(f"stream_bytes(B={B}, Fg={Fg}, max_chunk_frames={max_chunk_frames}): rejected ({n}); a cap below Fg needs "
+                             "the FP16 Generator")
+        return n
+
     def set_profiling(self, on: bool = True):
         self._check(self.lib.bv2_set_profiling(self._h, int(on)))
 
@@ -185,10 +204,12 @@ class Engine:
                 _ptr(attn), _ptr(y_mask), _ptr(z), _ptr(z_p), _ptr(m_p), _ptr(logs_p), self._stream()))
         return o, attn, y_mask, (z, z_p, m_p, logs_p)
 
-    def infer_finish_stream(self, B, T, F, noise_z, noise_scale, max_len=None, want_attn=True):
+    def infer_finish_stream(self, B, T, F, noise_z, noise_scale, max_len=None, want_attn=True, max_chunk_frames: Optional[int] = None):
         """infer_finish up to and including the flow, then open a Generator stream over the returned `o` [B,1,Fg*hop]; its samples become
         final as stream_advance() is called.  Returns (o, attn, y_mask, (z, z_p, m_p, logs_p)) like infer_finish.  Every precision;
-        no pcm16 (its peak normalisation needs the whole utterance)."""
+        no pcm16 (its peak normalisation needs the whole utterance).  `max_chunk_frames`: a cap on how far one stream_advance may
+        move the frontier; below Fg it bounds the stream's Generator memory (stream_bytes) and needs the FP16 Generator (ValueError
+        otherwise)."""
         I, hop = self.cfg.inter_channels, self.cfg.hop
         noise_z = self._f32(noise_z)
         assert noise_z.shape[0] == B and noise_z.shape[1] == I and noise_z.shape[2] >= F
@@ -199,15 +220,16 @@ class Engine:
         y_mask = torch.empty(B, 1, F, device=dev, dtype=torch.float32)
         z, z_p, m_p, logs_p = (torch.empty(B, I, F, device=dev, dtype=torch.float32) for _ in range(4))
         self._last = (B, T, F)
-        self._check(self.lib.bv2_infer_finish_stream(self._h, _ptr(noise_z), noise_z.shape[2], float(noise_scale),
-                                                     -1 if max_len is None else int(max_len), _ptr(o), _ptr(attn), _ptr(y_mask), _ptr(z),
-                                                     _ptr(z_p), _ptr(m_p), _ptr(logs_p), self._stream()))
+        self._check(self.lib.bv2_infer_finish_stream_bounded(self._h, _ptr(noise_z), noise_z.shape[2], float(noise_scale),
+                                                             -1 if max_len is None else int(max_len), _cap(max_chunk_frames), _ptr(o), _ptr(attn),
+                                                             _ptr(y_mask), _ptr(z), _ptr(z_p), _ptr(m_p), _ptr(logs_p), self._stream()))
         self._stream_o = o  # the stream writes into o until it closes
         return o, attn, y_mask, (z, z_p, m_p, logs_p)
 
     def stream_advance(self, frames: int) -> int:
         """Enqueue the Generator work that makes o[..., :min(frames, Fg)*hop] final on the current stream; returns that sample count.
-        Raises Bv2Error if no stream is open or `frames` does not exceed the frames already final."""
+        Raises Bv2Error if no stream is open or `frames` does not exceed the frames already final, and ValueError if the chunk exceeds a
+        bounded stream's max_chunk_frames (the stream stays open and unchanged)."""
         n = C.c_int64(0)
         self._check(self.lib.bv2_stream_advance(self._h, int(frames), self._stream(), C.byref(n)))
         return int(n.value)

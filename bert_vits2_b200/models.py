@@ -241,19 +241,25 @@ class SynthesizerTrn(nn.Module):
     @torch.no_grad()
     def infer_stream(self, x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_scale=0.667, length_scale=1,
                      noise_scale_w=0.8, max_len=None, sdp_ratio=0, y=None, *, noise_w=None, noise_z=None, w_ceil_override=None,
-                     first_chunk_frames=32):
+                     first_chunk_frames=32, max_chunk_frames=None):
         """Streaming infer(): a generator of waveform chunks o[:, :, a:b] (device tensors, views of one [B,1,Fg*hop] buffer) whose
         concatenation is bit-identical to infer(...)[0] with the same noise.  Encoder, durations and flow run whole first (the flow's
         attention spans the utterance); the Generator then runs as a wavefront, so the first chunk costs about first_chunk_frames
         + 14 frames of Generator work instead of all of it.  Chunks are first_chunk_frames frames, then double.  Each chunk is final
         when it is yielded (the host waits on an event recorded after its work) and no later chunk writes it.  Noise is drawn exactly
         as infer() draws it.  `last_y_lengths` is set before the first chunk.  There is no pcm16 option: the PCM conversion normalises by the peak of the whole utterance.
-        The generator leases one engine of the module's pool from its first step until it is exhausted, closed or collected."""
+        The generator leases one engine of the module's pool from its first step until it is exhausted, closed or collected.
+        `max_chunk_frames`: chunks double only up to this many frames, and the stream's Generator memory is then set by it, not by
+        the utterance's length (bounded stream: Engine.stream_bytes).  It needs the FP16 Generator (precision fp16 or fp16g) when it
+        is below the utterance's frame count; ValueError otherwise, and for max_chunk_frames < first_chunk_frames.  None: chunks
+        double without limit and every Generator activation stays resident until the stream ends."""
         dev = self._cuda_device("infer_stream")
         if x.dim() != 2 or bert.dim() != 3 or bert.shape[-1] != x.shape[1]:
             raise ValueError("expected x [B,T] and bert features [B,1024,T]")
         if first_chunk_frames < 1:
             raise ValueError("first_chunk_frames must be >= 1")
+        if max_chunk_frames is not None and max_chunk_frames < first_chunk_frames:
+            raise ValueError("max_chunk_frames must be >= first_chunk_frames")
         pool = self._pool(dev)
         B, T = x.shape
         eng = pool.acquire()
@@ -266,7 +272,8 @@ class SynthesizerTrn(nn.Module):
                                                length_scale, sdp_ratio, w_ceil_override)
                 if noise_z is None:
                     noise_z = torch.randn(B, self.inter_channels, F, device=dev, dtype=torch.float32)
-                o, _, _, _ = eng.infer_finish_stream(B, T, F, noise_z, noise_scale, max_len, want_attn=False)
+                cap = {} if max_chunk_frames is None else {"max_chunk_frames": max_chunk_frames}
+                o, _, _, _ = eng.infer_finish_stream(B, T, F, noise_z, noise_scale, max_len, want_attn=False, **cap)
                 results.append(o)
             eng._attn_token = object()  # a LazyAttn of an earlier infer() must not materialise this utterance's path
             self.last_y_lengths = y_lengths
@@ -281,7 +288,7 @@ class SynthesizerTrn(nn.Module):
                     ev.record(torch.cuda.current_stream(dev))
                     ev.synchronize()
                 yield o[:, :, done * hop:target * hop]
-                done, step = target, 2 * step
+                done, step = target, 2 * step if max_chunk_frames is None else min(2 * step, int(max_chunk_frames))
         finally:
             pool.release(eng)
 

@@ -129,6 +129,21 @@ int bv2_infer_finish_pcm16(bv2_engine* e, const float* noise_z, int64_t noise_ld
 int bv2_infer_finish_stream(bv2_engine* e, const float* noise_z, int64_t noise_ld, float noise_scale, int32_t max_len,
                             float* o, float* attn, float* y_mask, float* z, float* z_p, float* m_p, float* logs_p, void* stream);
 int bv2_stream_advance(bv2_engine* e, int32_t frames, void* stream, int64_t* samples_ready);
+/* Bounded stream: bv2_infer_finish_stream with a cap on how far one bv2_stream_advance may move the frontier.  With the FP16
+ * Generator (generator_precision 2 or 3) and max_chunk_frames in [1, Fg), each Generator tensor keeps only the rows later windows
+ * still read, in storage sized by the cap and not by Fg (bv2_stream_bytes), and the workspace the stream ensures is the encoder/flow
+ * part plus that storage.  Each advance may then launch one extra kernel that moves the live rows of the tensors it would overrun
+ * to the front of their storage, plus the conversion of the input rows the chunk reads; the audio stays bit-identical to
+ * bv2_infer_finish.  An advance with frames - (frames already final) > max_chunk_frames returns BV2_ERR_ARG and leaves the stream
+ * open and unchanged.  max_chunk_frames <= 0 or >= Fg: the unbounded stream of bv2_infer_finish_stream (which is this call with 0).
+ * On an fp32 or TF32 Generator a cap in [1, Fg) returns BV2_ERR_ARG. */
+int bv2_infer_finish_stream_bounded(bv2_engine* e, const float* noise_z, int64_t noise_ld, float noise_scale, int32_t max_len,
+                                    int32_t max_chunk_frames, float* o, float* attn, float* y_mask, float* z, float* z_p, float* m_p,
+                                    float* logs_p, void* stream);
+/* Workspace bytes of the Generator tensors of a stream over Fg frames of a batch of B with chunks of at most max_chunk_frames: for a
+ * cap in [1, Fg) the bounded storage, which does not depend on Fg; else what an unbounded stream allocates.  Negative (a BV2_ERR_*
+ * code) for bad arguments, an engine that is not finalized, or a cap in [1, Fg) on an fp32 / TF32 Generator. */
+int64_t bv2_stream_bytes(const bv2_engine* e, int B, int32_t Fg, int32_t max_chunk_frames);
 
 /* The same conversion for a waveform batch the caller already holds: wave [B,L] fp32 (device), n_valid [B] int64 (device,
  * may be NULL = L) -> out [B,L] int16 (device). */
@@ -142,6 +157,11 @@ int bv2_attn_path(bv2_engine* e, float* attn, void* stream);
 /* Size the workspace for batches up to (B, T tokens, F_cap frames) up front: afterwards no call within those bounds
  * allocates or synchronises the device (the workspace otherwise grows geometrically on first use of a larger shape). */
 int bv2_reserve(bv2_engine* e, int B, int T, int F_cap);
+/* bv2_reserve plus room for one stream with chunks of at most max_chunk_frames (<= 0: an unbounded stream) over up to F_cap frames:
+ * afterwards neither a call nor such a stream within those bounds grows the workspace.  A server reserves each engine of a pool
+ * for its largest shape and cap.  Like bv2_reserve, it closes an open stream when it regrows an arena.  A cap in [1, F_cap) on an
+ * fp32 / TF32 Generator returns BV2_ERR_ARG. */
+int bv2_reserve_stream(bv2_engine* e, int B, int T, int F_cap, int32_t max_chunk_frames);
 
 /* ---- per-stage entry points (parity tests + microbenchmarks; same kernels as the whole path) ---------------
  * text encoder: outputs x [B,H,T], m_p/logs_p [B,inter,T] (reference models.py:377-400)                       */
