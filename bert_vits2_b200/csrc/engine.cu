@@ -134,25 +134,26 @@ struct bv2_engine : DeviceWeights {
         float* gproj = nullptr; float* w_ceil = nullptr;
     } st;
     // Open Generator stream (bv2_infer_finish_stream .. the bv2_stream_advance that reaches Fg).  Every tensor of the Generator stays
-    // alive in the workspace for the stream's lifetime, because later windows read the rows behind each layer's done pointer: the
-    // input z plus conv_pre's output plus, per upsampling stage, the stage sum S, the upsampled xu and one tensor per resblock conv
-    // except the last of each chain (2 + 3 * (3 + 2) = 17 tensors per stage at the default configuration), against the one-shot
-    // Generator's per-stage release.  Per frame per utterance at the default configuration that is, besides z itself,
-    //   FP16 Generator (16-bit H8 tensors):  2 * (192 + 512 + 17 * (256*8 + 128*64 + 64*128 + 32*256 + 16*512)) = 1,185,152 bytes
-    //                                        plus the zero halo rows;
-    //   fp32 / TF32 Generator (fp32 c4):     4 * (512 + 17 * (256*8 + 128*64 + 64*128 + 32*256 + 16*512))       = 2,369,536 bytes.
+    // in the workspace for the stream's lifetime, because later windows read the rows behind each layer's done pointer: the input z
+    // plus conv_pre's output plus, per upsampling stage, the stage sum S, the upsampled xu and one tensor per resblock conv except the
+    // last of each chain (2 + 3 * (3 + 2) = 17 tensors per stage at the default configuration), against the one-shot Generator's
+    // per-stage release.
+    //   fp32 / TF32 Generator: whole fp32 c4 tensors, 4 * (512 + 17 * (256*8 + 128*64 + 64*128 + 32*256 + 16*512)) = 2,369,536 bytes
+    //                          per frame at the default configuration, besides z itself.
+    //   FP16 Generator: every tensor, the input included, is an H8 tensor of gen_stream_rows() rows of storage, and the input is
+    //                   converted from z chunk by chunk.  With chunks of at most max_chunk frames < Fg (a bounded stream) that is
+    //                   gen_stream_capacity(), independent of Fg, and a slide (k_g2_slide) moves a tensor's live rows to the front of its
+    //                   storage when a chunk would run past its end.  Otherwise every tensor is whole and never slides:
+    //                   2 * (192 + 512 + 17 * (256*8 + 128*64 + 64*128 + 32*256 + 16*512)) = 1,185,152 bytes per frame plus the halos.
     // The stream also reads the per-batch conditioning and the lengths in the persist arena.  Any call that resets the workspace, and a
     // bv2_reserve that regrows either arena, closes the stream.
-    // A bounded stream (FP16 Generator, chunks of at most max_chunk frames < Fg) keeps only the rows later windows still read: every
-    // H8 tensor, the input included, has gen_stream_capacity() rows of storage, independent of Fg, and a slide (k_g2_slide) moves a
-    // tensor's live rows to the front of its storage when a chunk would run past its end.  The input is converted from z chunk by chunk.
     struct {
         bool open = false; int B = 0, Fg = 0, frontier = 0;
         GenGraph g; std::vector<H8> t; std::vector<Act> a;  // tensors of the FP16 Generator (t) / of the fp32 c4 Generator (a)
         float* o = nullptr; const float* gdec = nullptr; int g_stride = 0; const int* lens = nullptr;
-        int max_chunk = 0;     // > 0: bounded stream
-        std::vector<int> cap;  // bounded: rows of storage per tensor (gen_stream_capacity)
-        Act z; const int* zlens = nullptr;  // bounded: the Generator input z (fp32 c4) and its lengths, converted per chunk
+        int max_chunk = 0;      // > 0: bounded stream
+        std::vector<int> rows;  // FP16: rows of storage per tensor (gen_stream_rows)
+        Act z;                  // FP16: the Generator input z (fp32 c4), converted per chunk
     } gs;
     void ws_reset() { gs.open = false; ws.reset(); }
     long long* h_ylen = nullptr;  // pinned: y_lengths[B <= 4096] + the input-validation mask
@@ -402,11 +403,8 @@ struct bv2_engine : DeviceWeights {
     void run_generator_g2(Act z, const int* lens_or_null, const float* gdec, int g_stride, float* o, cudaStream_t s);
     H8 g2_h8(int B, int C, int T, int rows = -1);
     H8 g2_input(Act z, const int* lens_or_null, cudaStream_t s);
-    int gen_channels(const GenGraph& g, int tensor) const;
-    size_t gen_stream_bytes(int B, int Fg) const;
-    bool stream_bounded(int Fg, int max_chunk) const { return use_g2 && max_chunk >= 1 && max_chunk < Fg; }
     size_t stream_bytes(int B, int Fg, int max_chunk) const;
-    void gen_stream_open(Act z, const int* lens_or_null, const float* gdec, int g_stride, float* o, int max_chunk, cudaStream_t s);
+    void gen_stream_open(Act z, const int* lens_or_null, const float* gdec, int g_stride, float* o, int max_chunk);
     void g2_stream_prepare(int done, int target, cudaStream_t s);
     void gen_windows(const GenGraph& g, const std::vector<GenWin>& w, std::vector<Act>& t, bool stream, const int* lens_or_null, const float* gdec,
                      int g_stride, float* o, cudaStream_t s);
@@ -1121,7 +1119,7 @@ void bv2_engine::run_generator_g2(Act z, const int* lens, const float* gdec, int
     g2_windows(g, gen_stream_plan(g, z.T, 0, z.T), t, false, gdec, g_stride, o, s);
 }
 
-// rows >= 0: storage for only that many rows (a bounded stream's tensor, H8::base); else the whole tensor
+// rows >= 0: storage for only that many rows (a stream's tensor, H8::base); else the whole tensor
 H8 bv2_engine::g2_h8(int B, int C, int T, int rows) {
     H8 t; t.B = B; t.C = C; t.T = T; t.Tp = G2_PADL + (rows >= 0 ? rows : T) + G2_PADR;
     t.p = reinterpret_cast<uint4*>(ws.alloc(H8::bytes(B, C, t.Tp - G2_PADL - G2_PADR) / 4)) + G2_PADL;
@@ -1136,66 +1134,47 @@ H8 bv2_engine::g2_input(Act z, const int* lens, cudaStream_t s) {
     return zh;
 }
 
-int bv2_engine::gen_channels(const GenGraph& g, int tensor) const {
-    if (tensor == 0) return cfg.inter_channels;
-    for (const GenLayer& l : g.layers)
-        if (l.out == tensor) return l.kind == GenLayer::CONV_PRE ? cfg.upsample_initial_channel : l.kind == GenLayer::CONV_POST ? 1 : ups[l.stage].Cout;
-    throw Error(BV2_ERR_INTERNAL, "gen_channels: unknown tensor");
-}
-
-// Workspace bytes of a stream's tensors (all but the waveform, which the caller owns, and, for the fp32 Generator, the input z,
-// which the caller allocated)
-size_t bv2_engine::gen_stream_bytes(int B, int Fg) const {
+// Workspace bytes of the tensors of a stream over Fg frames with chunks of at most max_chunk frames: all but the waveform, which the
+// caller owns, and, for the fp32 Generator, the input z, which the caller allocated.  Only the FP16 Generator bounds its storage, so a
+// cap below the frame count on any other is a BV2_ERR_ARG.
+size_t bv2_engine::stream_bytes(int B, int Fg, int max_chunk) const {
+    if (!use_g2 && gen_stream_bounded(Fg, max_chunk))
+        throw Error(BV2_ERR_ARG, "a chunk cap below the frame count needs the FP16 Generator (precision fp16 or fp16g)");
     const GenGraph g = gen_graph(cfg, Fg);
+    const std::vector<int> rows = gen_stream_rows(cfg, g, max_chunk);
     size_t n = 0;
-    for (size_t i = use_g2 ? 0 : 1; i + 1 < g.tensor_len.size(); i++) {
-        const int C = gen_channels(g, (int)i), L = g.tensor_len[i];
-        n += ((use_g2 ? H8::bytes(B, C, L) : (size_t)B * C * L * sizeof(float)) + 255) & ~(size_t)255;
+    for (size_t i = use_g2 ? 0 : 1; i + 1 < rows.size(); i++) {
+        const int C = g.tensor_ch[i];
+        n += ((use_g2 ? H8::bytes(B, C, rows[i]) : (size_t)B * C * rows[i] * sizeof(float)) + 255) & ~(size_t)255;
     }
     return n;
 }
 
-// Workspace bytes of a stream's Generator tensors with chunks of at most max_chunk frames: a bounded stream's storage (independent of
-// Fg), else gen_stream_bytes
-size_t bv2_engine::stream_bytes(int B, int Fg, int max_chunk) const {
-    if (!stream_bounded(Fg, max_chunk)) return gen_stream_bytes(B, Fg);
-    const GenGraph g = gen_graph(cfg, max_chunk + 1);  // channels only: they do not depend on the length
-    const std::vector<int> cap = gen_stream_capacity(cfg, max_chunk);
-    size_t n = 0;
-    for (size_t i = 0; i + 1 < cap.size(); i++) n += (H8::bytes(B, gen_channels(g, (int)i), cap[i]) + 255) & ~(size_t)255;
-    return n;
-}
-
-void bv2_engine::gen_stream_open(Act z, const int* lens, const float* gdec, int g_stride, float* o, int max_chunk, cudaStream_t s) {
+void bv2_engine::gen_stream_open(Act z, const int* lens, const float* gdec, int g_stride, float* o, int max_chunk) {
     gs.g = gen_graph(cfg, z.T);
     const size_t n = gs.g.tensor_len.size();
-    gs.t.clear(); gs.a.clear(); gs.cap.clear();
-    gs.max_chunk = stream_bounded(z.T, max_chunk) ? max_chunk : 0;
-    if (gs.max_chunk) {
-        gs.cap = gen_stream_capacity(cfg, gs.max_chunk);
+    gs.t.clear(); gs.a.clear(); gs.rows.clear();
+    if (use_g2) {
+        gs.rows = gen_stream_rows(cfg, gs.g, max_chunk);
         gs.t.assign(n, H8());
-        for (size_t i = 0; i + 1 < n; i++) gs.t[i] = g2_h8(z.B, gen_channels(gs.g, (int)i), gs.g.tensor_len[i], gs.cap[i]);
-        gs.z = z; gs.zlens = lens;
-    } else if (use_g2) {
-        gs.t.assign(n, H8());
-        gs.t[0] = g2_input(z, lens, s);
-        for (size_t i = 1; i + 1 < n; i++) gs.t[i] = g2_h8(z.B, gen_channels(gs.g, (int)i), gs.g.tensor_len[i]);
+        for (size_t i = 0; i + 1 < n; i++) gs.t[i] = g2_h8(z.B, gs.g.tensor_ch[i], gs.g.tensor_len[i], gs.rows[i]);
     } else {
         gs.a.assign(n, Act());
         gs.a[0] = z;
-        for (size_t i = 1; i + 1 < n; i++) gs.a[i] = ws.act(z.B, gen_channels(gs.g, (int)i), gs.g.tensor_len[i]);
+        for (size_t i = 1; i + 1 < n; i++) gs.a[i] = ws.act(z.B, gs.g.tensor_ch[i], gs.g.tensor_len[i]);
     }
-    gs.B = z.B; gs.Fg = z.T; gs.frontier = 0; gs.o = o; gs.gdec = gdec; gs.g_stride = g_stride; gs.lens = lens;
+    gs.max_chunk = gen_stream_bounded(z.T, max_chunk) ? max_chunk : 0;
+    gs.B = z.B; gs.Fg = z.T; gs.frontier = 0; gs.o = o; gs.gdec = gdec; gs.g_stride = g_stride; gs.lens = lens; gs.z = z;
     gs.open = true;
 }
 
-// Before the windows of the chunk done -> target of a bounded stream: one slide launch for the tensors whose storage the chunk would
-// overrun (gen_stream_slides), then the conversion of the input rows the chunk reads.
+// Before the windows of the chunk done -> target of an FP16 stream: one slide launch for the tensors whose storage the chunk would
+// overrun (gen_stream_slides; none while every tensor is whole), then the conversion of the input rows the chunk reads.
 void bv2_engine::g2_stream_prepare(int done, int target, cudaStream_t s) {
     const size_t n = gs.t.size();
     std::vector<int> base(n);
     for (size_t i = 0; i < n; i++) base[i] = gs.t[i].base;
-    const std::vector<GenSlide> sl = gen_stream_slides(gs.g, gs.Fg, gs.cap, base, done, target);
+    const std::vector<GenSlide> sl = gen_stream_slides(gs.g, gs.Fg, gs.rows, base, done, target);
     for (size_t k = 0; k < sl.size(); k += G2_SLIDE_MAX) {  // one launch at the default configuration (87 tensors)
         G2SlideParams sp{};
         int most = 0;
@@ -1211,7 +1190,7 @@ void bv2_engine::g2_stream_prepare(int done, int target, cudaStream_t s) {
     const int a = gen_needs(gs.g, gs.Fg, done).tensor[0], b = gen_needs(gs.g, gs.Fg, target).tensor[0];
     if (b > a) {
         const Act& z = gs.z;
-        k_c4_to_h8<<<dim3(cdiv(b - a, 128), z.C / 8, z.B), 128, 0, s>>>(reinterpret_cast<const float4*>(z.p), gs.t[0].p, z.C, z.T, gs.t[0].Tp, gs.zlens,
+        k_c4_to_h8<<<dim3(cdiv(b - a, 128), z.C / 8, z.B), 128, 0, s>>>(reinterpret_cast<const float4*>(z.p), gs.t[0].p, z.C, z.T, gs.t[0].Tp, gs.lens,
                                                                       a, b, gs.t[0].base);
         BV2_CUDA(cudaGetLastError()); launches++;
     }
@@ -1220,7 +1199,8 @@ void bv2_engine::g2_stream_prepare(int done, int target, cudaStream_t s) {
 // Runs every Generator layer over its window of w (GenGraph launch order; empty windows launch nothing) on the H8 tensors t, one per
 // GenGraph tensor.  stream = false: a one-shot run over whole layers; t holds only the input, and the stage temporaries are
 // bump-allocated per stage and released after the join (the convs of one resblock chain share one temporary and two ping-pong
-// buffers).  stream = true: a chunk of a stream, on tensors that live as long as the stream.
+// buffers).  stream = true: a chunk of a stream, on tensors that live as long as the stream and hold the rows of gen_stream_rows().
+// Every tensor is addressed by logical row through its base (0 for a whole tensor).
 void bv2_engine::g2_windows(const GenGraph& g, const std::vector<GenWin>& w, std::vector<H8>& t, bool stream, const float* gdec, int g_stride,
                             float* o, cudaStream_t s) {
     const int B = t[0].B;
@@ -1287,12 +1267,8 @@ void bv2_engine::g2_windows(const GenGraph& g, const std::vector<GenWin>& w, std
     const GenWin& wp = w[li];
     if (wp.t_end > wp.t_begin) {
         BV2_CHECK((x.base == 0 || wp.t_begin - 3 >= x.base) && std::min(wp.t_end + 3, x.T + G2_PADR) <= x.lim(), "conv_post input rows not resident");
-        const dim3 grid(cdiv(wp.t_end - wp.t_begin, 512), B);
-        if (x.base == 0 && x.Tp == G2_PADL + x.T + G2_PADR)
-            launch_pdl(k_conv_post_tanh_h8<16, 7>, grid, dim3(256), 0, s, (const uint4*)x.p, x.Tp, conv_post_h, o, lp.L_out, wp.t_begin, wp.t_end);
-        else  // a bounded stream's resident rows
-            launch_pdl(k_conv_post_tanh_h8_resident<16, 7>, grid, dim3(256), 0, s, (const uint4*)x.p, x.Tp, x.base, conv_post_h, o, lp.L_out, wp.t_begin,
-                       wp.t_end);
+        launch_pdl(k_conv_post_tanh_h8<16, 7>, dim3(cdiv(wp.t_end - wp.t_begin, 512), B), dim3(256), 0, s, (const uint4*)x.p, x.Tp, x.base, conv_post_h, o,
+                   lp.L_out, wp.t_begin, wp.t_end);
         launches++;
     }
 }
@@ -1330,8 +1306,7 @@ static size_t ws_bytes_for(const bv2_config& c, int B, int T, int F) { return ws
 // Workspace a stream over F frames (Fg of them through the Generator) ensures.  max_chunk <= 0: the unbounded stream, which has always
 // reserved the one-shot Generator's part as well; a cap: the encoder/flow part plus the stream's own tensors.
 static size_t ws_stream_bytes(const bv2_engine* e, int B, int T, int F, int Fg, int max_chunk) {
-    if (max_chunk <= 0) return ws_bytes_for(e->cfg, B, T, F) + e->gen_stream_bytes(B, Fg);
-    return ws_enc_flow_bytes(e->cfg, B, T, F) + e->stream_bytes(B, Fg, max_chunk);
+    return (max_chunk <= 0 ? ws_bytes_for(e->cfg, B, T, F) : ws_enc_flow_bytes(e->cfg, B, T, F)) + e->stream_bytes(B, Fg, max_chunk);
 }
 
 static size_t persist_bytes_for(const bv2_config& c, int B, int T, int gproj_n) {
@@ -1537,8 +1512,6 @@ static int infer_finish_impl(bv2_engine* e, const float* noise_z, int64_t noise_
     const bv2_config& c = e->cfg;
     const int B = st.B, T = st.T, F = st.F, I = c.inter_channels;
     const int Fg = (max_len > 0 && max_len < F) ? max_len : F;
-    if (open_stream && !e->use_g2 && max_chunk >= 1 && max_chunk < Fg)
-        throw Error(BV2_ERR_ARG, "a chunk cap below the frame count needs the FP16 Generator (precision fp16 or fp16g)");
     e->ws.ensure(open_stream ? ws_stream_bytes(e, B, T, F, Fg, max_chunk) : ws_bytes_for(c, B, T, F));
     e->ws_reset();
     float* m_tmp = m_p ? m_p : e->ws.alloc((size_t)B * I * F);
@@ -1571,7 +1544,7 @@ static int infer_finish_impl(bv2_engine* e, const float* noise_z, int64_t noise_
         BV2_CUDA(cudaMemcpy2DAsync(zg.p, (size_t)Fg * 16, z.p, (size_t)F * 16, (size_t)Fg * 16, (size_t)B * I / 4, cudaMemcpyDeviceToDevice, s));
     }
     if (open_stream) {
-        e->gen_stream_open(zg, st.ylen32, st.gproj + e->goff_dec, e->gproj_n, o, max_chunk, s);
+        e->gen_stream_open(zg, st.ylen32, st.gproj + e->goff_dec, e->gproj_n, o, max_chunk);
         st.active = false; st.finished = true;
         return BV2_OK;
     }
@@ -1627,9 +1600,12 @@ int bv2_stream_advance(bv2_engine* e, int32_t frames, void* stream, int64_t* sam
     const int f = std::min<int>(frames, gs.Fg);
     const std::vector<GenWin> w = gen_stream_plan(gs.g, gs.Fg, gs.frontier, f);
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (gs.max_chunk) e->g2_stream_prepare(gs.frontier, f, s);
-    if (e->use_g2) e->g2_windows(gs.g, w, gs.t, true, gs.gdec, gs.g_stride, gs.o, s);
-    else e->gen_windows(gs.g, w, gs.a, true, gs.lens, gs.gdec, gs.g_stride, gs.o, s);
+    if (e->use_g2) {
+        e->g2_stream_prepare(gs.frontier, f, s);
+        e->g2_windows(gs.g, w, gs.t, true, gs.gdec, gs.g_stride, gs.o, s);
+    } else {
+        e->gen_windows(gs.g, w, gs.a, true, gs.lens, gs.gdec, gs.g_stride, gs.o, s);
+    }
     gs.frontier = f;
     if (samples_ready) *samples_ready = (int64_t)f * e->hop;
     if (f == gs.Fg) gs.open = false;
@@ -1673,8 +1649,6 @@ static int reserve_impl(bv2_engine* e, int B, int T, int F_cap, bool with_stream
     BV2_API_BEGIN(e)
     BV2_CHECK(e->finalized && B >= 1 && T >= 1 && F_cap >= 1, "reserve args");
     const bv2_config& c = e->cfg;
-    if (with_stream && !e->use_g2 && max_chunk >= 1 && max_chunk < F_cap)
-        throw Error(BV2_ERR_ARG, "a chunk cap below the frame count needs the FP16 Generator (precision fp16 or fp16g)");
     const size_t need = reserve_bytes(e, B, T, F_cap, with_stream, max_chunk);
     const size_t pneed = persist_bytes_for(c, B, T, e->gproj_n);
     if (need > e->ws.cap() || pneed > e->persist.cap()) e->gs.open = false;  // regrowing an arena frees what an open stream reads
@@ -1693,10 +1667,10 @@ int64_t bv2_stream_bytes(const bv2_engine* e, int B, int32_t Fg, int32_t max_chu
     if (!e || !e->finalized || B < 1 || Fg < 1) return BV2_ERR_ARG;
     const int32_t cap = std::max<int32_t>(max_chunk_frames, 0);
     if (((int64_t)std::max(Fg, cap) + 1024) * e->hop > INT32_MAX) return BV2_ERR_ARG;  // rows of the waveform must fit an int
-    if (!e->use_g2 && cap >= 1 && cap < Fg) return BV2_ERR_ARG;
     try {
         return (int64_t)e->stream_bytes(B, Fg, cap);
-    } catch (const std::exception&) { return BV2_ERR_INTERNAL; }
+    } catch (const Error& ex) { return ex.code == BV2_ERR_ARG ? BV2_ERR_ARG : BV2_ERR_INTERNAL; }  // ARG: a cap the Generator cannot bound
+    catch (const std::exception&) { return BV2_ERR_INTERNAL; }
 }
 
 int bv2_text_encoder(bv2_engine* e, int B, int T, const int64_t* x, const int64_t* x_lengths, const int64_t* sid,

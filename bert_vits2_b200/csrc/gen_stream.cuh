@@ -31,7 +31,7 @@ struct GenLayer {
 };
 struct GenGraph {
     std::vector<GenLayer> layers;
-    std::vector<int> tensor_len;
+    std::vector<int> tensor_len, tensor_ch;  // rows and channels of each tensor
     int hop = 1;  // waveform samples per frame
 };
 struct GenWin { int t_begin = 0, t_end = 0; };  // output rows [t_begin, t_end); empty: no launch
@@ -40,23 +40,24 @@ constexpr int GEN_PRE_POST_REACH = 3;  // conv_pre and conv_post: 7 taps, paddin
 
 inline GenGraph gen_graph(const bv2_config& c, int Fg) {
     GenGraph g;
-    auto tensor = [&](int L) { g.tensor_len.push_back(L); return (int)g.tensor_len.size() - 1; };
+    auto tensor = [&](int L, int C) { g.tensor_len.push_back(L); g.tensor_ch.push_back(C); return (int)g.tensor_len.size() - 1; };
     auto layer = [&](int kind, int stage, int j, int d, int in, int out, int res, int reach, int u) {
         g.layers.push_back(GenLayer{kind, stage, j, d, in, out, res, reach, u, g.tensor_len[in], g.tensor_len[out]});
     };
-    int L = Fg;
-    const int z = tensor(L);
-    int x = tensor(L);
+    int L = Fg, C = c.upsample_initial_channel;
+    const int z = tensor(L, c.inter_channels);
+    int x = tensor(L, C);
     layer(GenLayer::CONV_PRE, -1, 0, 0, z, x, -1, GEN_PRE_POST_REACH, 1);
     for (int i = 0; i < c.n_ups; i++) {
         const int u = c.upsample_rates[i], Lo = L * u;
-        const int S = tensor(Lo), xu = tensor(Lo);
+        C /= 2;  // every upsampling stage halves the channels
+        const int S = tensor(Lo, C), xu = tensor(Lo, C);
         layer(GenLayer::UPS, i, 0, 0, x, xu, -1, ups_half(c.upsample_kernel_sizes[i], u), u);
         for (int j = 0; j < c.n_resblock_kernels; j++) {
             const int k = c.resblock_kernel_sizes[j];
             int cur = xu;
             for (int d = 0; d < c.n_dilations; d++) {
-                const int xt = tensor(Lo), nxt = d == c.n_dilations - 1 ? S : tensor(Lo);
+                const int xt = tensor(Lo, C), nxt = d == c.n_dilations - 1 ? S : tensor(Lo, C);
                 layer(GenLayer::RB_C1, i, j, d, cur, xt, -1, (k - 1) / 2 * c.resblock_dilation_sizes[j][d], 1);
                 layer(GenLayer::RB_C2, i, j, d, xt, nxt, cur, (k - 1) / 2, 1);
                 cur = nxt;
@@ -64,7 +65,7 @@ inline GenGraph gen_graph(const bv2_config& c, int Fg) {
         }
         x = S; L = Lo; g.hop *= u;
     }
-    layer(GenLayer::CONV_POST, -1, 0, 0, x, tensor(L), -1, GEN_PRE_POST_REACH, 1);
+    layer(GenLayer::CONV_POST, -1, 0, 0, x, tensor(L, 1), -1, GEN_PRE_POST_REACH, 1);
     return g;
 }
 
@@ -141,10 +142,22 @@ inline std::vector<int> gen_stream_capacity(const bv2_config& c, int max_chunk_f
     }
 }
 
+// A stream over Fg frames is bounded when its chunk cap lies in [1, Fg).
+inline bool gen_stream_bounded(int Fg, int max_chunk_frames) { return max_chunk_frames >= 1 && max_chunk_frames < Fg; }
+
+// Rows of storage of every tensor of a stream over g (Fg = g.tensor_len[0] frames) with chunks of at most max_chunk_frames: the
+// capacities of a bounded stream, else every tensor whole (L rows, so gen_stream_slides never slides it).  The waveform gets 0.
+inline std::vector<int> gen_stream_rows(const bv2_config& c, const GenGraph& g, int max_chunk_frames) {
+    if (gen_stream_bounded(g.tensor_len[0], max_chunk_frames)) return gen_stream_capacity(c, max_chunk_frames);
+    std::vector<int> rows(g.tensor_len);
+    rows.back() = 0;
+    return rows;
+}
+
 // One slide: rows [src, src + rows) of every row block of tensor `tensor` move to [dst, dst + rows) (physical rows, dst < src).
 struct GenSlide { int tensor, src, dst, rows; };
 
-// Slides that let the chunk done -> target fit in the capacities cap (gen_stream_capacity), given the current bases (updated in place;
+// Slides that let the chunk done -> target fit in the storage rows cap (gen_stream_rows), given the current bases (updated in place;
 // the waveform, the last tensor, is never bounded).  A tensor slides only when the chunk's rows would run past its storage; its base
 // then becomes resident_begin(done) and the final rows it still reads, [resident_begin(done), need(done)), move to the front.
 inline std::vector<GenSlide> gen_stream_slides(const GenGraph& g, int Fg, const std::vector<int>& cap, std::vector<int>& base, int done, int target) {

@@ -353,14 +353,15 @@ __global__ void __launch_bounds__(128) k_c4_to_h8(const float4* __restrict__ x, 
 // kernel parameters (constant bank: FFMA takes them as an operand), and a thread's inner loop is one conflict-free LDS + one FFMA per tap.
 template <int C, int K> struct PostW { float w[C * K]; };  // [C][K]
 // Outputs [t_begin, t_end) of the T samples are stored; staged rows past t_end feed discarded outputs only.  x holds the logical rows
-// [x_base, row_end) (H8::base); rows from row_end on are read as zero.
+// from x_base (H8::base; 0 for a whole tensor) to the end of its storage; rows from the halo's end T + G2_PADR on, or from the storage's
+// end if that comes first, are read as zero.
 template <int C, int K>
-__device__ __forceinline__ void conv_post_tanh_h8(const uint4* __restrict__ x, int Tp, int x_base, int row_end, const PostW<C, K>& pw,
-                                                  float* __restrict__ y, int T, int t_begin, int t_end) {
+__global__ void __launch_bounds__(256) k_conv_post_tanh_h8(const uint4* __restrict__ x, int Tp, int x_base, const __grid_constant__ PostW<C, K> pw,
+                                                           float* __restrict__ y, int T, int t_begin, int t_end) {
     constexpr int TB = 512, RW = TB + K - 1, LD = RW + 2;  // outputs per block, staged rows, row stride of the staged tile
     __shared__ float sx[C][LD];
     asm volatile("griddepcontrol.wait;" ::: "memory");
-    const int t0 = t_begin + blockIdx.x * TB, b = blockIdx.y;
+    const int t0 = t_begin + blockIdx.x * TB, b = blockIdx.y, row_end = min(T + G2_PADR, x_base + Tp - G2_PADL);
     for (int i = threadIdx.x; i < (C / 8) * RW; i += blockDim.x) {
         const int g = i / RW, r = i - g * RW, row = t0 - K / 2 + r;  // row >= -K/2 >= -G2_PADL
         float f[8];
@@ -387,18 +388,6 @@ __device__ __forceinline__ void conv_post_tanh_h8(const uint4* __restrict__ x, i
         }
         if (t < t_end) y[(size_t)b * T + t] = tanhf(acc);
     }
-}
-// A whole H8 input (rows [-G2_PADL, T + G2_PADR) allocated)
-template <int C, int K>
-__global__ void __launch_bounds__(256) k_conv_post_tanh_h8(const uint4* __restrict__ x, int Tp, const __grid_constant__ PostW<C, K> pw, float* __restrict__ y, int T,
-                                                           int t_begin, int t_end) {
-    conv_post_tanh_h8<C, K>(x, Tp, 0, T + G2_PADR, pw, y, T, t_begin, t_end);
-}
-// The input of a bounded stream (H8 with base x_base): rows past the storage's end read as zero like the halo past T + G2_PADR
-template <int C, int K>
-__global__ void __launch_bounds__(256) k_conv_post_tanh_h8_resident(const uint4* __restrict__ x, int Tp, int x_base, const __grid_constant__ PostW<C, K> pw,
-                                                                    float* __restrict__ y, int T, int t_begin, int t_end) {
-    conv_post_tanh_h8<C, K>(x, Tp, x_base, min(T + G2_PADR, x_base + Tp - G2_PADL), pw, y, T, t_begin, t_end);
 }
 
 // Slide of a bounded stream (gen_stream_slides): for each descriptor, rows [src, src + rows) of every one of its `blocks` row blocks

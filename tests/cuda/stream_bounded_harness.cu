@@ -105,7 +105,7 @@ int kh_conv_post_resident(const void* x, int x_base, int x_rows, const float* w,
         uint8_t* dy = ar.guarded(y, yb);
         PostW<16, 7> pw;
         std::memcpy(pw.w, w, sizeof(pw.w));
-        launch_pdl(k_conv_post_tanh_h8_resident<16, 7>, dim3(cdiv(t_end - t_begin, 512), B), dim3(256), 0, (cudaStream_t)0, (const uint4*)xx.p, xx.Tp, xx.base, pw,
+        launch_pdl(k_conv_post_tanh_h8<16, 7>, dim3(cdiv(t_end - t_begin, 512), B), dim3(256), 0, (cudaStream_t)0, (const uint4*)xx.p, xx.Tp, xx.base, pw,
                    reinterpret_cast<float*>(dy), T, t_begin, t_end);
         finish(err_flag);
         *guard_ok = read_guarded(dy, y, yb);

@@ -79,7 +79,7 @@ int kh_conv_post_window(const void* x, const float* w, int B, int T, int t_begin
         uint8_t* dy = ar.guarded(y, yb);
         PostW<16, 7> pw;
         std::memcpy(pw.w, w, sizeof(pw.w));
-        launch_pdl(k_conv_post_tanh_h8<16, 7>, dim3(cdiv(t_end - t_begin, 512), B), dim3(256), 0, (cudaStream_t)0, (const uint4*)xx.p, xx.Tp, pw,
+        launch_pdl(k_conv_post_tanh_h8<16, 7>, dim3(cdiv(t_end - t_begin, 512), B), dim3(256), 0, (cudaStream_t)0, (const uint4*)xx.p, xx.Tp, 0, pw,
                    reinterpret_cast<float*>(dy), T, t_begin, t_end);
         finish(err_flag);
         *guard_ok = read_guarded(dy, y, yb);
