@@ -16,15 +16,17 @@
 //     per element, and conv zero padding is the tensor's own zero halo (no per-tile fill, no predicates);
 //   * tap j of a dilated conv is the same staged tile with the descriptor start advanced by j*dil rows (as in tc_conv.cuh).
 //
-// One kernel, k_g2_conv: a CTA owns a super-tile of NG x MG m-tiles (128 rows each) x nt <= 128 columns, NG*MG*nt <= 128 columns of
-// fp32 accumulator image in shared memory (the whole accumulator of the super-tile), so each weight stage (chunk c, tap j) feeds MG
-// 128-row MMAs:
+// One kernel, k_g2_conv: a CTA owns a super-tile of NG groups x MG m-tiles (128 rows each) x nt <= 128 columns, NG*MG*nt <= 128
+// columns; each weight stage (chunk c, tap j) feeds MG 128-row MMAs:
 //   streamed weights (C >= 64): NG = 1, MG = 128/nt -- weights cross L2->SM once per MG*128 rows, ring of up to 16 stages;
 //   resident weights (C <= 32): all taps loaded once, the M-groups pipeline through the activation ring and the tail of
 //   group g overlaps the MMAs of group g+1.
-// 640 threads: warp 0 activation producer, warp 2 weight producer, warp 3 output halo, warps 16-19 MMA warpgroup (warp 1 idle),
-// warps 4-15 epilogue (accumulator init with the bias before the MMAs; tail accumulator image -> [+ residual] [+ MRF running sum] -> lrelu -> f16
-// -> 16-byte coalesced stores).
+// A group's fp32 accumulators live in the wgmma registers of two MMA warpgroups (64 rows of every m-tile each, MG*nt/2 <= 64
+// registers per thread) from the bias to the last k-step, one wgmma group in flight behind the one being issued; at the group's end they
+// are written once into the group's columns of an fp32 image in shared memory ([column][ACC_TS rows], NG*MG*nt columns), which the
+// epilogue reads.
+// 640 threads: warp 0 activation producer, warp 2 weight producer, warp 3 output halo (warp 1 idle), warps 4-11 epilogue (accumulator
+// image -> [+ residual] [+ MRF running sum] -> lrelu -> f16 -> 16-byte coalesced stores), warps 12-19 the two MMA warpgroups.
 #pragma once
 #include "tc_conv.cuh"
 
@@ -65,63 +67,106 @@ __device__ __forceinline__ void unpack8(const uint4& u, float* f) {
 __device__ __forceinline__ float unlrelu10(float a) { return a >= 0.f ? a : a * 10.f; }
 }  // namespace tc
 
-// MMAs of one weight stage (chunk c, tap j): MG m-tiles x NK k-steps (NK compile-time), each m-tile one wg_mma over the
-// accumulator image.
-template <int NK, int MG>
-__device__ __forceinline__ void g2_issue_stage(uint32_t d0, uint32_t a_lo0, uint32_t b_lo0, uint32_t a_kstep, uint32_t b_kstep, uint64_t hi, uint32_t nt) {
-#pragma unroll 1
-    for (int mt = 0; mt < MG; mt++)
-        tc::wg_mma<1>(d0 + (uint32_t)mt * nt, hi | (a_lo0 + (uint32_t)(mt * 128)), hi | b_lo0, a_kstep, b_kstep, NK, (int)nt, 1u);
-}
-
-// State the MMA issuer carries through its loops (all warp-uniform)
+// State the MMA issuer carries through its loops (all warpgroup-uniform except img, the thread's own fragment rows)
 struct G2Issue {
     uint32_t bar_af, bar_ae, bar_wf, bar_we, bar_acc;      // first barrier of each group
-    uint32_t a_lo_base, w_lo_base, a_stage16, w_stage16;   // descriptor low words of ring slot 0, slot strides (16-byte units)
-    uint32_t a_kstep, b_kstep, nt, dil, tm;
+    uint32_t a_lo_base, w_lo_base, a_stage16, w_stage16;   // descriptor low words of ring slot 0 (A: this warpgroup's 64 rows), slot strides (16-byte units)
+    uint32_t a_kstep, b_kstep, dil;
     uint32_t nas, nws;
     int NG, NCH, K, streamed;
     uint64_t hi;
+    const float* sbias;                                    // the N tile's bias (+ per-batch bias) row, staged in shared memory
+    float* img;                                            // accumulator image at (row of this thread's first fragment row, column 0)
 };
 
-// The issuer's loop nest for one (NK, MG) instantiation.  Ring slots, parities, barrier addresses and descriptor words are carried
+// Arrive on an mbarrier from thread 0 of the warpgroup if bar != 0 (bar = 0: nothing to release).  One asm block: a C++ branch here
+// would make ptxas serialise the wgmma pipeline across it.
+__device__ __forceinline__ void g2_release(uint32_t bar) {
+    asm volatile("{\n\t.reg .pred p, e;\n\t.reg .u32 t;\n\tmov.u32 t, %%tid.x;\n\tand.b32 t, t, 127;\n\tsetp.eq.u32 e, t, 0;\n\t"
+                 "setp.ne.and.u32 p, %0, 0, e;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}" ::"r"(bar) : "memory");
+}
+
+// The issuer's loop nest for one (NK, MG, NT) instantiation, run by each of the two MMA warpgroups on its 64 rows of every m-tile.
+// A group's accumulators stay in registers (MG x NT/2 fp32 per thread, indexed by compile-time constants only) from the bias to the
+// last k-step; the accumulator image is written once per group, for the epilogue.  Per output the fp32 sequence is bias, then chunk c,
+// tap j, k-step, whatever the tiling.  Each stage's MMAs are one wgmma group; once the previous group has completed (wait_group 1), its
+// ring slots are released while the current one runs.  Ring slots, parities, barrier addresses and descriptor words are carried
 // incrementally (adds and compares only: no runtime integer division in front of every stage's MMAs).
-template <int NK, int MG>
+template <int NK, int MG, int NT>
 __device__ __forceinline__ void g2_issuer(const G2Issue& q) {
     using namespace tc;
+    float acc[MG][NT / 2];
+    const int cq = 2 * (threadIdx.x & 3);
     uint32_t sa = 0, aph = 0, a_cur = q.a_lo_base;   // activation ring slot, parity, descriptor low word of the slot
     uint32_t sw = 0, wph = 0, w_cur = q.w_lo_base;   // weight ring (streamed) / tap cursor (resident)
-    uint32_t dg = q.tm;
-    for (int g = 0; g < q.NG; g++, dg += (uint32_t)MG * q.nt) {
-        if (!q.streamed) w_cur = q.w_lo_base;
+    for (int g = 0; g < q.NG; g++) {
+        // bias (+ per-batch bias): thread columns 8 i + cq (+1) of every m-tile, rows r and r + 8
+#pragma unroll
+        for (int i = 0; i < NT / 8; i++) {
+            const float2 b2 = *reinterpret_cast<const float2*>(q.sbias + 8 * i + cq);
+#pragma unroll
+            for (int mt = 0; mt < MG; mt++) { acc[mt][4 * i] = b2.x; acc[mt][4 * i + 1] = b2.y; acc[mt][4 * i + 2] = b2.x; acc[mt][4 * i + 3] = b2.y; }
+        }
+        if (!q.streamed) {
+            if (g == 0) mbar_wait_u(q.bar_wf, 0);  // all taps, loaded once
+            w_cur = q.w_lo_base;
+        }
+        uint32_t rel_w = 0, rel_a = 0;  // slots the previous stage read: released once its MMAs have completed
         for (int c = 0; c < q.NCH; c++) {
             mbar_wait_u(q.bar_af + 8u * sa, aph);
             uint32_t a_tap = a_cur;
             for (int j = 0; j < q.K; j++, a_tap += q.dil) {
                 if (q.streamed) mbar_wait_u(q.bar_wf + 8u * sw, wph);
-                g2_issue_stage<NK, MG>(dg, a_tap, w_cur, q.a_kstep, q.b_kstep, q.hi, q.nt);
-                if (q.streamed) wg_commit(q.bar_we + 8u * sw);
+                wgmma_fence();
+#pragma unroll
+                for (int mt = 0; mt < MG; mt++)
+#pragma unroll
+                    for (int kk = 0; kk < NK; kk++)
+                        Wgmma<1, NT>::mma(acc[mt], q.hi | (a_tap + (uint32_t)(mt * 128) + (uint32_t)kk * q.a_kstep), q.hi | (w_cur + (uint32_t)kk * q.b_kstep));
+                wgmma_commit();
+                wgmma_wait1();
+                g2_release(rel_w);
+                g2_release(rel_a);
+                rel_w = q.streamed ? q.bar_we + 8u * sw : 0u;
+                rel_a = j == q.K - 1 ? q.bar_ae + 8u * sa : 0u;
                 w_cur += q.w_stage16;
                 if (q.streamed && ++sw == q.nws) { sw = 0; wph ^= 1u; w_cur = q.w_lo_base; }
             }
-            wg_commit(q.bar_ae + 8u * sa);
             a_cur += q.a_stage16;
             if (++sa == q.nas) { sa = 0; aph ^= 1u; a_cur = q.a_lo_base; }
         }
-        wg_commit(q.bar_acc + 8u * (uint32_t)g);
+        wgmma_wait0();
+        g2_release(rel_w);
+        g2_release(rel_a);
+        // hand-off: the group's columns of the image (same fragment-to-image map as tc::wg_slice), then one arrival per thread
+        float* im = q.img + (size_t)(g * MG * NT + cq) * ACC_TS;
+#pragma unroll
+        for (int mt = 0; mt < MG; mt++) {
+#pragma unroll
+            for (int i = 0; i < NT / 8; i++) {
+                float* d = im + (size_t)(mt * NT + 8 * i) * ACC_TS;
+                d[0] = acc[mt][4 * i]; d[ACC_TS] = acc[mt][4 * i + 1]; d[8] = acc[mt][4 * i + 2]; d[ACC_TS + 8] = acc[mt][4 * i + 3];
+            }
+        }
+        mbar_arrive(q.bar_acc + 8u * (uint32_t)g);
     }
 }
-// MG dispatch as a binary tree of two-way branches (a switch would become a jump table: BRX on a vector register makes ptxas treat
-// the code after it as divergent and takes the descriptors out of the uniform datapath)
-template <int NK>
+// (NT, MG) dispatch as a binary tree of two-way branches (a switch would become a jump table: BRX on a vector register makes ptxas treat
+// the code after it as divergent and takes the descriptors out of the uniform datapath).  Only MG * NT <= 128 is instantiated: the
+// planner never exceeds 128 accumulator columns per group.
+template <int NK, int NT, int LO, int HI>
 __device__ __forceinline__ void g2_issuer_mg(const G2Issue& q, int MG) {
-    if (MG <= 4) {
-        if (MG <= 2) { if (MG == 1) g2_issuer<NK, 1>(q); else g2_issuer<NK, 2>(q); }
-        else { if (MG == 3) g2_issuer<NK, 3>(q); else g2_issuer<NK, 4>(q); }
-    } else {
-        if (MG <= 6) { if (MG == 5) g2_issuer<NK, 5>(q); else g2_issuer<NK, 6>(q); }
-        else { if (MG == 7) g2_issuer<NK, 7>(q); else g2_issuer<NK, 8>(q); }
+    if constexpr (LO == HI) g2_issuer<NK, LO, NT>(q);
+    else {
+        constexpr int MID = (LO + HI) / 2;
+        if (MG <= MID) g2_issuer_mg<NK, NT, LO, MID>(q, MG);
+        else g2_issuer_mg<NK, NT, MID + 1, HI>(q, MG);
     }
+}
+template <int NK>
+__device__ __forceinline__ void g2_issuer_nt(const G2Issue& q, int nt, int MG) {
+    if (nt <= 32) { if (nt == 16) g2_issuer_mg<NK, 16, 1, 8>(q, MG); else g2_issuer_mg<NK, 32, 1, 4>(q, MG); }
+    else { if (nt == 64) g2_issuer_mg<NK, 64, 1, 2>(q, MG); else g2_issuer<NK, 1, 128>(q); }
 }
 
 __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
@@ -137,19 +182,21 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
     uint64_t* bars = reinterpret_cast<uint64_t*>(sW + (size_t)nwst * p.w_stage_bytes);
     const uint32_t bar0 = smem_u32(bars);
     auto BAR = [&](int i) { return bar0 + 8u * (uint32_t)i; };
-    // barrier map: a_full[NAS], a_empty[NAS], w_full[NWS], w_empty[NWS], acc_full[NG], acc_init
-    const int B_AFULL = 0, B_AEMPTY = NAS, B_WFULL = 2 * NAS, B_WEMPTY = 2 * NAS + NWS, B_ACC = 2 * NAS + 2 * NWS, B_INIT = B_ACC + NG;
+    // barrier map: a_full[NAS], a_empty[NAS], w_full[NWS], w_empty[NWS], acc_full[NG]
+    const int B_AFULL = 0, B_AEMPTY = NAS, B_WFULL = 2 * NAS, B_WEMPTY = 2 * NAS + NWS, B_ACC = 2 * NAS + 2 * NWS;
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < NAS; i++) { mbar_init(BAR(B_AFULL + i), 1); mbar_init(BAR(B_AEMPTY + i), 1); }
-        for (int i = 0; i < NWS; i++) { mbar_init(BAR(B_WFULL + i), 1); mbar_init(BAR(B_WEMPTY + i), 1); }
-        for (int i = 0; i < NG; i++) mbar_init(BAR(B_ACC + i), 1);
-        mbar_init(BAR(B_INIT), 12 * 32);
+        // a ring slot is free once both MMA warpgroups released it; a group's image is complete once all 256 MMA threads stored theirs
+        for (int i = 0; i < NAS; i++) { mbar_init(BAR(B_AFULL + i), 1); mbar_init(BAR(B_AEMPTY + i), 2); }
+        for (int i = 0; i < NWS; i++) { mbar_init(BAR(B_WFULL + i), 1); mbar_init(BAR(B_WEMPTY + i), 2); }
+        for (int i = 0; i < NG; i++) mbar_init(BAR(B_ACC + i), 256);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
     const uint32_t acc0 = 0;  // accumulator image base (acc_ptr)
     const int ncg = p.KC / 8;  // 16-byte channel groups per chunk
+    // registers: the producer warpgroup (warps 0-3) hands registers to the MMA warpgroups, which hold up to 64 fp32 accumulators per
+    // thread on top of their loop state (40 x 128 + 96 x 256 + 120 x 256 <= the 96 x 640 the CTA is launched with)
 
     if (warp == 0) {
         // ===== activation producer (reads the upstream kernel's output: PDL wait first)
@@ -161,7 +208,7 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
             const int row0 = t0 + g * MG * 128 - p.pad;
             const int nrows = max(0, min(R, p.x_lim - row0));  // never read past the tensor's halo or storage; rows beyond (and rows past a window's end) feed discarded outputs only
             if (lane == 0) {
-                mbar_wait(BAR(B_AEMPTY + sa), ((s / NAS) & 1) ^ 1);
+                mbar_wait_u(BAR(B_AEMPTY + sa), ((s / NAS) & 1) ^ 1);
                 mbar_expect_tx(BAR(B_AFULL + sa), (uint32_t)nrows * 16u * (uint32_t)ncg);
             }
             __syncwarp();
@@ -196,29 +243,40 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
                 }
             }
         }
-    } else if (warp >= 16) {
+    } else if (warp >= 12) {
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-        // ===== MMA warpgroup (warps 16-19): all 128 threads run the loops together (wgmma is warpgroup-collective)
+        // ===== two MMA warpgroups (warps 12-15: rows 0-63, warps 16-19: rows 64-127 of every m-tile): all 128 threads of a warpgroup
+        // run the loops together (wgmma is warpgroup-collective)
         // Descriptors are kept as (constant high word, 32-bit low word): start address >> 4 in bits [0,14), LBO >> 4 in [16,30) of the low
         // word; tap / m-tile / k-step offsets are plain 32-bit adds on the low word (shared memory addresses stay below 2^18), which the
         // compiler keeps in the uniform datapath.
+        const int wg = (warp - 12) >> 2;
         const uint32_t a_lo_c = (((uint32_t)R * 16u) >> 4) << 16, b_lo_c = (((uint32_t)nt * 16u) >> 4) << 16;
         const uint32_t desc_hi = 128u >> 4;  // SBO = 128 B
-        const uint32_t a_kstep = 2u * (uint32_t)R, b_kstep = 2u * (uint32_t)nt;
-        const uint32_t tm = acc0;
         const int nk = p.KC / 16;
-        if (p.resident) mbar_wait_u(BAR(B_WFULL), 0);
-        mbar_wait_u(BAR(B_INIT), 0);  // accumulators hold the bias: every MMA accumulates
         G2Issue q;
         q.bar_af = BAR(B_AFULL); q.bar_ae = BAR(B_AEMPTY); q.bar_wf = BAR(B_WFULL); q.bar_we = BAR(B_WEMPTY); q.bar_acc = BAR(B_ACC);
-        q.a_lo_base = ((smem_u32(sA) & 0x3ffffu) >> 4) | a_lo_c; q.w_lo_base = ((smem_u32(sW) & 0x3ffffu) >> 4) | b_lo_c;
+        q.a_lo_base = (((smem_u32(sA) & 0x3ffffu) >> 4) + 64u * (uint32_t)wg) | a_lo_c;  // + 64 rows x 16 B per warpgroup
+        q.w_lo_base = ((smem_u32(sW) & 0x3ffffu) >> 4) | b_lo_c;
         q.a_stage16 = p.a_stage_bytes >> 4; q.w_stage16 = p.w_stage_bytes >> 4;
-        q.a_kstep = a_kstep; q.b_kstep = b_kstep; q.nt = (uint32_t)nt; q.dil = (uint32_t)p.dil; q.tm = tm;
+        q.a_kstep = 2u * (uint32_t)R; q.b_kstep = 2u * (uint32_t)nt; q.dil = (uint32_t)p.dil;
         q.nas = (uint32_t)NAS; q.nws = (uint32_t)NWS; q.NG = NG; q.NCH = NCH; q.K = p.K;
         q.streamed = !p.resident;
         q.hi = (uint64_t)desc_hi << 32;
-        if (nk == 2) g2_issuer_mg<2>(q, MG);
-        else g2_issuer_mg<1>(q, MG);  // g2_conv() admits KC = 16 or 32 only
+        q.img = acc_ptr(acc0) + 64 * wg + 16 * (warp & 3) + (lane >> 2);
+        // the N tile's bias row (+ this batch's per-batch bias), staged once: every group starts its fragment from it
+        float* sbias = reinterpret_cast<float*>(bars + B_ACC + NG);
+        const int tb = threadIdx.x - 384;
+        if (tb < nt) {
+            const int n = n0 + tb;
+            float bv = __ldg(p.bias + (p.ups_u ? n % p.ups_cout : n));
+            if (p.bias_b) bv += __ldg(p.bias_b + (size_t)b * p.bias_b_stride + n);
+            sbias[tb] = bv;
+        }
+        asm volatile("bar.sync 1, 256;" ::: "memory");  // the two MMA warpgroups
+        q.sbias = sbias;
+        if (nk == 2) g2_issuer_nt<2>(q, nt, MG);
+        else g2_issuer_nt<1>(q, nt, MG);  // g2_conv() admits KC = 16 or 32 only
     } else if (warp == 3) {
         // ===== zero halo of the OUTPUT tensor (= the conv padding of its consumers), written by its producer: the CTA of the first super-tile
         // clears rows [-G2_PADL, 0) if the window starts at t = 0, the CTA of the last one rows [T_out, T_out + G2_PADR) if the window ends at
@@ -235,45 +293,21 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
             if (hi)
                 for (int i = lane; i < p.y_cg * G2_PADR; i += 32) yb[(size_t)(i / G2_PADR) * p.y_Tp + Tout + (i % G2_PADR)] = z4;
         }
-    } else if (warp >= 4 && warp < 16) {
-        // ===== epilogue, 12 warps: row quarter q = warp & 3; the 3 warps of a quarter share the (m-tile, 32-column batch) items
-        // round-robin.  Two phases:
-        //   init (before the MMAs, before the PDL wait: touches only static data and the CTA-private accumulator image): the accumulators are pre-loaded
-        //        with bias (+ per-batch bias) by image stores, so every MMA accumulates and the tail has no bias loads / adds;
-        //   tail: the accumulator image -> [+ residual] [+ MRF running sum] -> lrelu -> f16 -> coalesced 16-byte stores.
+    } else if (warp >= 4) {
+        // ===== epilogue, 8 warps (4-11): row quarter q = warp & 3; the 2 warps of a quarter share the (m-tile, 32-column batch) items
+        // round-robin.  The accumulator image of a group (bias included: the MMA warpgroups start from it) -> [+ residual]
+        // [+ MRF running sum] -> lrelu -> f16 -> coalesced 16-byte stores.
         // The tail is instruction-bound (two-three warps per scheduler cannot hide ALU latency: round-2 ncu), so it is kept lean.
         asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
         const int e = warp - 4, q = warp & 3, part = e >> 2;
         const uint32_t trow = acc0 + ((uint32_t)(q * 32) << 16);
         const int u = p.ups_u;
         const int ncb = nt >= 32 ? nt / 32 : 1, cw = nt >= 32 ? 32 : 16;  // column batches per m-tile, columns per batch
-        {
-            for (int cb = part; cb < ncb; cb += 3) {
-                const int col0 = cb * cw;
-                uint32_t v[32];
-#pragma unroll
-                for (int h = 0; h < 8; h++) {
-                    if (4 * h < cw) {
-                        const int n = n0 + col0 + 4 * h;
-                        float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + (u ? n % p.ups_cout : n)));
-                        if (p.bias_b) {
-                            const float4 c4 = __ldg(reinterpret_cast<const float4*>(p.bias_b + (size_t)b * p.bias_b_stride + n));
-                            b4.x += c4.x; b4.y += c4.y; b4.z += c4.z; b4.w += c4.w;
-                        }
-                        v[4 * h] = __float_as_uint(b4.x); v[4 * h + 1] = __float_as_uint(b4.y); v[4 * h + 2] = __float_as_uint(b4.z); v[4 * h + 3] = __float_as_uint(b4.w);
-                    }
-                }
-                for (int m = 0; m < NG * MG; m++) {
-                    if (cw == 32) acc_st<32>(trow + (uint32_t)(m * nt + col0), v); else acc_st<16>(trow + (uint32_t)(m * nt + col0), v);
-                }
-            }
-            mbar_arrive(BAR(B_INIT));
-        }
         asm volatile("griddepcontrol.wait;" ::: "memory");
         const bool scaled = p.out_scale != 1.f;
         for (int g = 0; g < NG; g++) {
-            mbar_wait(BAR(B_ACC + g), 0);
-            for (int it = part; it < MG * ncb; it += 3) {
+            mbar_wait_u(BAR(B_ACC + g), 0);
+            for (int it = part; it < MG * ncb; it += 2) {
                 const int mt = it / ncb, col0 = (it - mt * ncb) * cw;
                 const int t = t0 + (g * MG + mt) * 128 + q * 32 + lane;
                 const bool ok = t < p.t_end;  // stores, residual reads and running-sum updates stay inside the window
@@ -493,6 +527,9 @@ inline G2Plan g2_conv_plan(const TcConvW& w, const float* bias, const H8& x, con
         while (MG > 1 && 2 * a_bytes(MG) + 4 * (size_t)p.w_stage_bytes + 1024 > budget) MG--;
     }
     MG = std::min(MG, 8);
+    // the MMA warpgroups hold a group's MG x nt accumulator columns in registers: k_g2_conv is instantiated for nt in {16, 32, 64, 128}
+    // and MG * nt <= 128
+    BV2_CHECK((w.nt == 16 || w.nt == 32 || w.nt == 64 || w.nt == 128) && MG * w.nt <= 128, "g2_conv N tile");
     p.NG = NG; p.MG = MG; p.R = MG * 128 + halo;
     p.a_stage_bytes = (uint32_t)a_bytes(MG);
     const int a_steps = NG * w.nchunks;
@@ -505,7 +542,8 @@ inline G2Plan g2_conv_plan(const TcConvW& w, const float* bias, const H8& x, con
     else p.nws = (int)std::max<size_t>(2, std::min<size_t>(16, (budget - (size_t)nas * p.a_stage_bytes - 1024) / p.w_stage_bytes));
     if (!p.resident) p.nws = std::min(p.nws, NG * w.nchunks * w.K);
     p.acc_cols = (uint32_t)(NG * MG * w.nt);
-    const size_t smem = tc::acc_img_bytes(p.acc_cols) + (size_t)nas * p.a_stage_bytes + (p.resident ? w_all : (size_t)p.nws * p.w_stage_bytes) + (size_t)(2 * nas + 2 * p.nws + NG + 3) * 8 + 16;
+    const size_t smem = tc::acc_img_bytes(p.acc_cols) + (size_t)nas * p.a_stage_bytes + (p.resident ? w_all : (size_t)p.nws * p.w_stage_bytes) +
+                        (size_t)(2 * nas + 2 * p.nws + NG + 3) * 8 + (size_t)w.nt * 4 + 16;  // barriers, bias row
     BV2_CHECK(smem <= 227 * 1024, "g2_conv shared memory");
     G2Plan pl;
     pl.resident = p.resident; pl.NG = NG; pl.MG = MG; pl.nas = nas; pl.nws = p.nws; pl.smem = smem;
