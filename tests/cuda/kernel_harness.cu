@@ -253,6 +253,25 @@ int kh_g2_conv(const KhG2Args* a, void* y, KhG2Plan* plan, int* guard_ok, int* e
     });
 }
 
+// ---- Generator input conversion ------------------------------------------------------------------------------------------
+// k_c4_to_h8 as the engine launches it: rows [t_begin, t_end) of x (fp32 c4 [B][C/4][T][4], rows t >= lens[b] read as zero) into an
+// H8 whose storage holds `rows` logical rows from y_base on (y: [B][C/8][G2_PADL + rows + G2_PADR][8] halves, in = initial contents).
+int kh_c4_to_h8(const float* x, const int* lens, int B, int C, int T, int t_begin, int t_end, int y_base, int rows, void* y, int* guard_ok,
+                int* err_flag) {
+    return guarded_call([&] {
+        init_device();
+        BV2_CHECK(C % 8 == 0 && 0 <= y_base && y_base <= t_begin && t_begin < t_end && t_end <= T && t_end - y_base <= rows, "c4_to_h8 window");
+        Arena ar;
+        const size_t yb = H8::bytes(B, C, rows);
+        uint8_t* dy = ar.guarded(y, yb);
+        k_c4_to_h8<<<dim3(cdiv(t_end - t_begin, 128), C / 8, B), 128>>>(reinterpret_cast<const float4*>(ar.up(x, (size_t)B * C * T)),
+                                                                       reinterpret_cast<uint4*>(dy) + G2_PADL, C, T, G2_PADL + rows + G2_PADR,
+                                                                       ar.up(lens, (size_t)B), t_begin, t_end, y_base);
+        finish(err_flag);
+        *guard_ok = read_guarded(dy, y, yb);
+    });
+}
+
 const char* kh_last_error() { return g_err.c_str(); }
 int kh_g2_padl() { return G2_PADL; }
 int kh_g2_padr() { return G2_PADR; }

@@ -1,6 +1,8 @@
 """Case matrix of the kernel tests: every tensor-core conv call shape the engine makes with the default model config (with the engine's
-N tile / K chunk), at the edges where tiling goes wrong, plus num_sms values that force each dispatch branch of tc_conv1d.
-Shared by tests/test_kernels_cpu.py (dispatch coverage through the host planner) and tests/test_kernels_gpu.py (H100 runs)."""
+N tile / K chunk), at the edges where tiling goes wrong, plus num_sms values that force each dispatch branch of tc_conv1d; every
+k_g2_conv plan the FP16 Generator can select, found by search through the host planner; the fp32 Generator's SIMT conv cases.
+Shared by tests/test_kernels_cpu.py and tests/test_gen_kernels_cpu.py (coverage through the host planner) and
+tests/test_kernels_gpu.py and tests/test_gen_kernels_gpu.py (H100 runs)."""
 import numpy as np
 
 import kernel_harness as KH
@@ -123,26 +125,216 @@ def attn_cases():
     return out
 
 
-# ---- Generator conv (k_g2_conv): (id, Cin, Cout, K, dil, u, T, B, res, acc, scale, st_override, bias_b)
+# ---- Generator conv (k_g2_conv)
+# A plan key names the code a k_g2_conv launch runs: (NK = K chunk / 16, N tile, MG m-tiles per group, resident weights, NG groups per CTA).
+# The MMA issuer is one template instantiation per (NK, MG, NT); NG and the weight mode select the pipeline around it.
+def g2_key(p):
+    return (p.kc // 16, p.nt, p.MG, p.resident, p.NG)
+
+
+def g2_key_name(k):
+    nk, nt, mg, res, ng = k
+    return f"{'nk2-' if nk == 2 else ''}nt{nt}-mg{mg}-ng{ng}-{'res' if res else 'str'}"
+
+
+# the issuer instantiations k_g2_conv compiles (g2_issuer_nt): NK in {1, 2}, NT in {16, 32, 64, 128}, MG * NT <= 128, MG <= 8
+G2_ISSUERS = [(nk, nt, mg) for nk in (1, 2) for nt in (16, 32, 64, 128) for mg in range(1, min(8, 128 // nt) + 1)]
+
+
+def g2_layers(cfg=None):
+    """The FP16 Generator's k_g2_conv launches at a model configuration (default: ModelConfig()), one dict per layer: the layer's name,
+    the arguments the planner reads (Cin, Cout, K, u, dil) and the epilogue the engine gives it (bb: conv_pre's per-batch bias;
+    res: every convs2 adds the chain's input; acc / scale: the last convs2 of MRF branch j > 0 accumulates into the stage sum, the last
+    branch scaled by 1 / n_kernels).  The layer list comes from the Generator graph the engine walks (tests/cuda/stream_harness.cu)."""
+    import stream_harness as SH
+    from bert_vits2_b200.spec import ModelConfig
+    cfg = cfg or ModelConfig()
+    nk, nd = len(cfg.resblock_kernel_sizes), len(cfg.resblock_dilation_sizes[0])
+    out = []
+    for l in SH.Graph(cfg, 1).layers:
+        kind, i, j, d = SH.KINDS[l["kind"]], l["stage"], l["branch"], l["dil_idx"]
+        C = cfg.upsample_initial_channel >> (i + 1)
+        f = dict(name=kind, Cin=C, Cout=C, K=0, u=0, dil=1, bb=0, res=0, acc=0, scale=1.0)
+        if kind == "conv_pre":
+            f.update(Cin=cfg.inter_channels, Cout=cfg.upsample_initial_channel, K=7, bb=1)
+        elif kind == "ups":
+            f.update(name=f"ups{i}", Cin=2 * C, K=cfg.upsample_kernel_sizes[i], u=l["u"])
+        elif kind in ("c1", "c2"):
+            K = cfg.resblock_kernel_sizes[j]
+            f.update(name=f"s{i}_{kind}_k{K}_n{d}", K=K)  # n: position in the dilation chain
+            if kind == "c1":
+                f["dil"] = cfg.resblock_dilation_sizes[j][d]
+            else:
+                f["res"] = 1
+                if d == nd - 1:
+                    f.update(acc=int(j > 0), scale=1.0 / nk if j == nk - 1 else 1.0)
+        else:
+            continue  # conv_post: k_conv_post_tanh_h8
+        out.append(f)
+    return out
+
+
+def g2_epilogue(f):
+    """short name of a layer's engine epilogue: pre (per-batch bias), ups, c1 (plain), c2 (residual), c2acc (+ running sum), c2acc3 (+ 1/3)"""
+    if f["bb"]:
+        return "pre"
+    if f["u"]:
+        return "ups"
+    if not f["res"]:
+        return "c1"
+    return "c2" + ("acc" if f["acc"] else "") + ("3" if f["scale"] != 1.0 else "")
+
+
+def g2_layer_plan(f, T, B, num_sms, st=0):
+    return KH.g2_plan(KH.g2_args(B=B, T=T, Cin=f["Cin"], Cout=f["Cout"], K=f["K"], u=f["u"], dil=f["dil"], residual=f["res"],
+                                 accumulate=f["acc"], out_scale=f["scale"], st_override=st, num_sms=num_sms, res=1 if f["res"] else None,
+                                 bias_b=1 if f["bb"] else None, bias_b_stride=f["Cout"] + 40 if f["bb"] else 0))
+
+
+def g2_reachable(cfg=None, batches=range(1, 33), sms_list=(132, 114)):
+    """{plan key: (layer, T, B, num_sms)} of every plan the engine can select for the Generator of cfg: every layer, batch size and
+    SM count, over every window length (the planner sees the m-tiles of a window, so T = 128 * m-tiles) from one m-tile up to where the
+    super-tile saturates at 128 / nt m-tiles.  Beyond that the plan no longer changes: the resident group choice then compares
+    candidates that all cover 128 / nt m-tiles.  The example kept per key is the first found with the fewest rows (B * T)."""
+    KH.load()
+    seen, reach = set(), {}
+    for f in g2_layers(cfg):
+        sig = (f["Cin"], f["Cout"], f["K"], f["u"], f["dil"])  # all the planner reads besides T, B, num_sms
+        if sig in seen:
+            continue
+        seen.add(sig)
+        p1 = g2_layer_plan(f, 128, 1, 132)
+        mgmax, ntiles = max(1, 128 // p1.nt), p1.grid_y
+        for sms in sms_list:
+            for B in batches:
+                sat = max(2, -(-((mgmax - 1) * sms + 1) // (ntiles * B)))
+                for m in range(1, sat + 1):
+                    k = g2_key(g2_layer_plan(f, 128 * m, B, sms))
+                    if k not in reach or B * m < reach[k][2] * reach[k][1] // 128:
+                        reach[k] = (f, 128 * m, B, sms)
+    return reach
+
+
+# (T, B, num_sms, st_override) candidates of the case search, cheapest first: B * T small, the engine's own planning (st_override = 0)
+# before forced super-tiles, the H100's SM count before small ones (3 SMs: several waves at a few m-tiles, which decides between
+# pipelines of equal size)
+G2_SEARCH_SMS = (132, 114, 3)
+
+
+def _g2_candidates(mgmax):
+    out = []
+    for m in range(1, 25):
+        for B in (1, 2):
+            for si, sms in enumerate(G2_SEARCH_SMS):
+                for st in range(0, mgmax + 1):
+                    out.append(((B * m, B, st > 0, si, st), m, B, sms, st))
+    return [c[1:] for c in sorted(out)]
+
+
+def _g2_shape_ok(p, m, need):
+    """need = "tail": every group of every CTA holds rows (m-tiles a multiple of the super-tile); "partial": several CTAs, the last
+    one's super-tile partial -- with NG > 1, at least one whole group of it past the end"""
+    st = p.NG * p.MG
+    rem = m - (p.grid_x - 1) * st
+    if need == "tail":
+        return m % st == 0
+    if p.grid_x < 2:
+        return False
+    if p.NG > 1:
+        return rem <= (p.NG - 1) * p.MG
+    return rem < st or st == 1
+
+
+def g2_generated_cases(cfg=None):
+    """Cases found by search over every Generator layer of cfg (one per layer shape and engine epilogue) and the candidates above:
+    for each plan key the search reaches, a "tail" case and a "partial" case on the first layer that reaches it, and one tail case for
+    every other engine epilogue that reaches it.  T is never a multiple of 128: tail cases end 45 rows into their last m-tile, partial
+    cases 28 rows into it, so the groups past the end start >= 32 rows past the last halo row (their activation copy is 0 bytes) even
+    at the largest conv padding (25 rows).  Returns (id, Cin, Cout, K, dil, u, T, B, res, acc, scale, st_override, bias_b, num_sms, key)."""
+    KH.load()
+    found = {}  # (key, epilogue, need) -> (cost, case)
+    order = []  # keys in the order first reached
+    shapes = {}
+    for f in g2_layers(cfg):
+        shapes.setdefault((f["Cin"], f["Cout"], f["K"], f["u"], f["dil"], g2_epilogue(f)), f)
+    for f in shapes.values():
+        ep = g2_epilogue(f)
+        mgmax = max(1, 128 // g2_layer_plan(f, 128, 1, 132).nt)
+        for m, B, sms, st in _g2_candidates(mgmax):
+            p = g2_layer_plan(f, 128 * m, B, sms, st)
+            k = g2_key(p)
+            if k not in order:
+                order.append(k)
+            for need, T in (("tail", 128 * m - 45), ("partial", 128 * (m - 1) + 28)):
+                if T < 1 or (k, ep, need) in found or not _g2_shape_ok(p, m, need):
+                    continue
+                found[(k, ep, need)] = (B * T * f["Cin"] * f["Cout"] * f["K"], f, T, B, sms, st)
+    out = []
+    for k in order:
+        eps = sorted({ep for kk, ep, _ in found if kk == k}, key=lambda ep: min(found[(k, ep, n)][0] for n in ("tail", "partial")
+                                                                                 if (k, ep, n) in found))
+        for i, ep in enumerate(eps):
+            for need in ("tail", "partial") if i == 0 else ("tail",):
+                if (k, ep, need) not in found:
+                    continue
+                _, f, T, B, sms, st = found[(k, ep, need)]
+                out.append((f"plan-{g2_key_name(k)}-{ep}-{need}", f["Cin"], f["Cout"], f["K"], f["dil"], f["u"], T, B, f["res"], f["acc"],
+                            f["scale"], st, f["bb"], sms, k))
+    return out
+
+
+_g2_cases = None
+
+
 def g2_cases():
+    """(id, Cin, Cout, K, dil, u, T, B, res, acc, scale, st_override, bias_b, num_sms, expected plan key or None)"""
+    global _g2_cases
+    if _g2_cases is not None:
+        return _g2_cases
     base = [  # the shape matrix: every tail, edge tiles, both weight modes
         (16, 16, 3, 1, 0, 300, 1, 0, 0, 1.0, 0), (16, 16, 11, 5, 0, 1000, 2, 1, 0, 1.0, 0), (16, 16, 7, 3, 0, 5000, 1, 1, 1, 1 / 3, 0),
         (32, 32, 11, 5, 0, 3000, 1, 1, 0, 1.0, 0), (32, 32, 3, 1, 0, 129, 3, 1, 1, 1.0, 0), (64, 64, 7, 3, 0, 2000, 1, 1, 0, 1.0, 0),
         (64, 64, 11, 1, 0, 700, 2, 0, 0, 1.0, 3), (128, 128, 3, 1, 0, 1000, 1, 1, 0, 1.0, 4), (128, 128, 11, 5, 0, 600, 1, 1, 1, 1 / 3, 2),
         (256, 256, 7, 3, 0, 500, 1, 1, 0, 1.0, 2), (192, 512, 7, 1, 0, 300, 2, 0, 0, 1.0, 0),
         (512, 256, 16, 1, 8, 200, 1, 0, 0, 1.0, 0), (128, 64, 8, 1, 2, 700, 2, 0, 0, 1.0, 0), (32, 16, 8, 1, 2, 3000, 1, 0, 0, 1.0, 0),
+        # the engine's ups1 (256 -> 128, K 16, u 8) and ups4 (32 -> 16 at K 2, u 2)
+        (256, 128, 16, 1, 8, 300, 1, 0, 0, 1.0, 0), (32, 16, 2, 1, 2, 1000, 2, 0, 0, 1.0, 0),
     ]
-    out = [(f"probe-{i}", *c, 0) for i, c in enumerate(base)]
+    out = [(f"probe-{i}", *c, 0, H100_SMS, None) for i, c in enumerate(base)]
     # every super-tile override of a streamed and a resident layer, T at the 128-row tile edges
     # (streamed layers hold at most 128 / nt m-tiles of accumulators: MG <= 2 at C = 64)
     for st in (1, 2):
-        out.append((f"st{st}-streamed-C64-T1000", 64, 64, 11, 1, 0, 1000, 1, 1, 0, 1.0, st, 0))
+        out.append((f"st{st}-streamed-C64-T1000", 64, 64, 11, 1, 0, 1000, 1, 1, 0, 1.0, st, 0, H100_SMS, None))
     for st in (1, 2, 3, 4, 8):
-        out.append((f"st{st}-resident-C32-T3000", 32, 32, 11, 5, 0, 3000, 1, 1, 1, 1 / 3, st, 0))
+        out.append((f"st{st}-resident-C32-T3000", 32, 32, 11, 5, 0, 3000, 1, 1, 1, 1 / 3, st, 0, H100_SMS, None))
     for T in (1, 127, 128, 129, 255, 257):
-        out.append((f"edge-C64-K11d5-T{T}", 64, 64, 11, 5, 0, T, 2, 1, 1, 1 / 3, 0, 0))
-        out.append((f"edge-C16-K3-T{T}", 16, 16, 3, 1, 0, T, 1, 1, 0, 1.0, 0, 0))
+        out.append((f"edge-C64-K11d5-T{T}", 64, 64, 11, 5, 0, T, 2, 1, 1, 1 / 3, 0, 0, H100_SMS, None))
+        out.append((f"edge-C16-K3-T{T}", 16, 16, 3, 1, 0, T, 1, 1, 0, 1.0, 0, 0, H100_SMS, None))
     for T in (1, 129, 1000):  # conv_pre with the per-batch (speaker) bias
-        out.append((f"conv_pre-bias_b-T{T}", 192, 512, 7, 1, 0, T, 2, 0, 0, 1.0, 0, 1))
-    out.append(("ups-K2u2-C64-T129", 64, 32, 2, 1, 2, 129, 1, 0, 0, 1.0, 0, 0))
+        out.append((f"conv_pre-bias_b-T{T}", 192, 512, 7, 1, 0, T, 2, 0, 0, 1.0, 0, 1, H100_SMS, None))
+    out.append(("ups-K2u2-C64-T129", 64, 32, 2, 1, 2, 129, 1, 0, 0, 1.0, 0, 0, H100_SMS, None))
+    # every plan the engine's layers can reach, with each epilogue the engine gives them
+    out += g2_generated_cases()
+    _g2_cases = out
     return out
+
+
+# ---- fp32 Generator (SIMT kernels)
+def conv1d_big_tile(T, Cout, B):
+    """the tile launch_conv1d_k picks: 128 x 64 when that grid has >= 96 CTAs, else 16 x 16 with the 4-way split of the reduction"""
+    return -(-T // 128) * -(-Cout // 64) * B >= 96
+
+
+# k_conv1d_c4 (resblock convs, lrelu 0.1 input): (id, C, K, dil, T, B, residual, accumulate with out_scale 1/3).  Each K runs both tiles.
+CONV1D_CASES = [
+    ("C16-k3d1-res-T300-B2", 16, 3, 1, 300, 2, 1, 0),
+    ("C64-k7d3-acc-T129-B1", 64, 7, 3, 129, 1, 0, 1),
+    ("C256-k11d5-res-acc-T200-B2", 256, 11, 5, 200, 2, 1, 1),
+    ("C256-k3d5-T37-B1", 256, 3, 5, 37, 1, 0, 0),
+    ("C64-k3d3-res-acc-T6150-B2", 64, 3, 3, 6150, 2, 1, 1),
+    ("C256-k7d1-res-T1537-B2", 256, 7, 1, 1537, 2, 1, 0),
+    ("C16-k11d5-acc-T6100-B2", 16, 11, 5, 6100, 2, 0, 1),
+    ("C256-k11d1-T1600-B2", 256, 11, 1, 1600, 2, 0, 0),
+]
+# k_convT_c4 at the three ups geometries (K, u) of the default config, Cin = 2 Cout as every upsampling stage
+CONVT_CASES = [(f"K{K}u{u}-C{Co}-T{T}", K, u, Co, T) for K, u in ((16, 8), (8, 2), (2, 2)) for Co in (16, 64, 256) for T in (1, 15, 16, 17, 100)]

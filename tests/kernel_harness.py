@@ -68,6 +68,7 @@ def load(build=True):
         h.kh_flow_attn.argtypes = [P, P, P, P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, P, I, I, I]
         h.kh_g2_plan.argtypes = [C.POINTER(G2Args), C.POINTER(G2Plan)]
         h.kh_g2_conv.argtypes = [C.POINTER(G2Args), P, C.POINTER(G2Plan), I, I]
+        h.kh_c4_to_h8.argtypes = [P, P] + [C.c_int] * 7 + [P, I, I]
         h.kh_last_error.restype = C.c_char_p
         _lib_h = h
     return _lib_h
@@ -177,3 +178,16 @@ def g2_conv(args, y_init):
     p, g, e = G2Plan(), C.c_int(0), C.c_int(0)
     _check(load().kh_g2_conv(C.byref(args), y.ctypes.data, C.byref(p), C.byref(g), C.byref(e)))
     return y, p, bool(g.value), e.value
+
+
+def c4_to_h8(x_c4, lens, B, Cc, T, t_begin, t_end, y_base, y_init):
+    """k_c4_to_h8 over rows [t_begin, t_end) into an H8 holding the logical rows from y_base (y_init: [B][C/8][PADL + rows + PADR][8] f16);
+    returns (y after the kernel, guards intact, device error flag)"""
+    pl, pr = g2_pads()
+    y = np.array(y_init, np.float16, copy=True)
+    x_c4 = np.ascontiguousarray(x_c4, np.float32)
+    lens = np.ascontiguousarray(lens, np.int32)
+    g, e = C.c_int(0), C.c_int(0)
+    _check(load().kh_c4_to_h8(x_c4.ctypes.data, lens.ctypes.data, B, Cc, T, int(t_begin), int(t_end), int(y_base), y.shape[2] - pl - pr,
+                              y.ctypes.data, C.byref(g), C.byref(e)))
+    return y, bool(g.value), e.value

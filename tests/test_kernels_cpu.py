@@ -142,10 +142,12 @@ def test_n_tile_widths_of_the_case_matrix():
 def test_g2_plan_cases_reach_both_weight_modes_and_super_tiles():
     KH.load()
     modes, mgs = set(), set()
-    for cid, Cin, Cout, K, dil, u, T, B, res, acc, scale, st, bb in KC.g2_cases():
+    for cid, Cin, Cout, K, dil, u, T, B, res, acc, scale, st, bb, sms, expect in KC.g2_cases():
         p = KH.g2_plan(KH.g2_args(B=B, T=T, Cin=Cin, Cout=Cout, K=K, u=u, dil=dil, residual=res, accumulate=acc, out_scale=scale,
-                                  st_override=st, num_sms=KC.H100_SMS, res=1 if res else None, bias_b=1 if bb else None,
+                                  st_override=st, num_sms=sms, res=1 if res else None, bias_b=1 if bb else None,
                                   bias_b_stride=Cout + 40 if bb else 0))
+        if expect:
+            assert KC.g2_key(p) == expect, (cid, KC.g2_key_name(expect), str(p))
         modes.add(p.resident)
         mgs.add((p.resident, p.NG, p.MG))
     assert modes == {0, 1}

@@ -16,24 +16,13 @@ import pytest
 import kernel_cases as KC
 import kernel_harness as KH
 import kernel_ref as R
+from util import report
 
 pytestmark = pytest.mark.gpu
 
 
 def _rng(cid):
     return np.random.default_rng(zlib.crc32(cid.encode()))
-
-
-def _report(cid, plan, err, tol, mag, ok_mask, coords):
-    """prints the case line (plan, worst err/mag) and fails with the location and plan of the worst element"""
-    ratio = np.where(ok_mask, err / np.maximum(tol, 1e-30), 0.0)
-    bad = ok_mask & ~(err <= tol)
-    emag = float(np.max(np.where(ok_mask & (mag > 0), err / np.maximum(mag, 1e-30), 0.0))) if ok_mask.any() else 0.0
-    print(f"\n  {cid}: {plan} | worst err/mag {emag:.2e}, worst err/tol {float(ratio.max()) if ratio.size else 0.0:.3f}")
-    if bad.any():
-        idx = np.unravel_index(np.argmax(ratio), ratio.shape)
-        pytest.fail(f"{cid}: {int(bad.sum())} element(s) out of bound; worst at {coords}={tuple(int(i) for i in idx)}: "
-                    f"err {float(err[idx]):.3e} > tol {float(tol[idx]):.3e} (mag {float(mag[idx]):.3e}); plan {plan}")
 
 
 # ------------------------------------------------------------------------------------------------------------ tc_conv1d
@@ -109,7 +98,7 @@ def test_tc_conv1d(cid, fam, B, T, lens, sms, expect):
         f"{cid}: channels outside the output window changed; plan {plan}"
     got = y[:, win].astype(np.float64)
     assert np.isfinite(got).all(), f"{cid}: non-finite outputs at (b, c, t)={tuple(int(i) for i in np.argwhere(~np.isfinite(got))[0])}; plan {plan}"
-    _report(cid, plan, np.abs(got - ref["ref"]), ref["tol"], ref["mag"], np.ones(got.shape, bool), "(b, c, t)")
+    report(cid, plan, np.abs(got - ref["ref"]), ref["tol"], ref["mag"], np.ones(got.shape, bool), "(b, c, t)")
 
 
 # ------------------------------------------------------------------------------------------------------------ fused flow attention
@@ -163,13 +152,13 @@ def test_flow_attention(cid, B, T, lens, ks, planted):
     # max|Ev|) + fp32 scores / ex2.approx (<< 2^-11): ~1e-3 (max|v| + max|Ev|); 4e-3 leaves 4x margin.  Rows >= len: exact zeros.
     valid = (np.arange(T)[None, :] < np.asarray(lens)[:, None])[:, None, :, None]
     tol = np.where(valid, 4e-3 * (np.abs(v).max() + np.abs(ev).max()), 0.0) * np.ones_like(ref)
-    _report(cid, plan, np.abs(got - ref), tol, np.full(ref.shape, np.abs(v).max() + np.abs(ev).max()), np.ones(ref.shape, bool),
+    report(cid, plan, np.abs(got - ref), tol, np.full(ref.shape, np.abs(v).max() + np.abs(ev).max()), np.ones(ref.shape, bool),
             "(b, head, t, d)")
 
 
 # ------------------------------------------------------------------------------------------------------------ Generator conv (H8)
-@pytest.mark.parametrize("cid,Cin,Cout,K,dil,u,T,B,res,acc,scale,st,bb", KC.g2_cases(), ids=[c[0] for c in KC.g2_cases()])
-def test_g2_conv(cid, Cin, Cout, K, dil, u, T, B, res, acc, scale, st, bb):
+@pytest.mark.parametrize("cid,Cin,Cout,K,dil,u,T,B,res,acc,scale,st,bb,sms,expect", KC.g2_cases(), ids=[c[0] for c in KC.g2_cases()])
+def test_g2_conv(cid, Cin, Cout, K, dil, u, T, B, res, acc, scale, st, bb, sms, expect):
     g = _rng(cid)
     To = T * max(1, u)
     act = lambda s: R.f16(R.lrelu32(g.standard_normal(s).astype(np.float32), 0.1))  # stored Generator activations
@@ -185,16 +174,18 @@ def test_g2_conv(cid, Cin, Cout, K, dil, u, T, B, res, acc, scale, st, bb):
     yh = KH.to_h8(y_old if acc else np.full((B, Cout, To), np.nan, np.float32), np.nan)  # halos NaN: the kernel must zero them
     arrs = [np.ascontiguousarray(v) for v in (w, bias)]
     args = KH.g2_args(B=B, T=T, Cin=Cin, Cout=Cout, K=K, u=u, dil=dil, residual=res, accumulate=acc, out_scale=scale, st_override=st,
-                      num_sms=KC.H100_SMS, w=arrs[0].ctypes.data, bias=arrs[1].ctypes.data, x=xh.ctypes.data,
+                      num_sms=sms, w=arrs[0].ctypes.data, bias=arrs[1].ctypes.data, x=xh.ctypes.data,
                       res=rh.ctypes.data if res else None, bias_b=bias_b.ctypes.data if bb else None,
                       bias_b_elems=bias_b.size if bb else 0, bias_b_stride=stride if bb else 0)
     out1, plan, guard1, err1 = KH.g2_conv(args, yh)
     out2, _, guard2, err2 = KH.g2_conv(args, yh)
     assert err1 == 0 and err2 == 0, f"{cid}: device error flag raised; plan {plan}"
     assert guard1 and guard2, f"{cid}: guard region around the output overwritten; plan {plan}"
+    if expect:
+        assert KC.g2_key(plan) == expect, (cid, KC.g2_key_name(expect), str(plan))
     assert out1.tobytes() == out2.tobytes(), f"{cid}: second run not bitwise identical; plan {plan}"
     data, halo = KH.h8_data(out1)
     assert (halo == 0).all(), f"{cid}: halo rows of the output not zero after the conv; plan {plan}"
     assert np.isfinite(data).all(), f"{cid}: non-finite outputs; plan {plan}"
     ref = R.g2_conv(a, w, bias, u=u, dil=dil, bias_b=None if bias_b is None else bias_b[:, :Cout], res=r, y_old=y_old, out_scale=scale)
-    _report(cid, plan, np.abs(data.astype(np.float64) - ref["ref"]), ref["tol"], ref["mag"], np.ones(data.shape, bool), "(b, c, t)")
+    report(cid, plan, np.abs(data.astype(np.float64) - ref["ref"]), ref["tol"], ref["mag"], np.ones(data.shape, bool), "(b, c, t)")

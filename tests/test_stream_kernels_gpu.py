@@ -12,20 +12,22 @@ from stream_harness import conv1d_window, conv_post_simt_window, conv_post_windo
 
 pytestmark = pytest.mark.gpu
 
-# (name, Cin, Cout, K, u, dil, mode, st_override): the Generator's conv shapes of the default configuration
+# (name, Cin, Cout, K, u, dil, mode, st_override, T, (NG, MG) of the whole launch or None): the Generator's conv shapes of the default
+# configuration; the forced super-tiles are those of a long utterance's stage 4 (NG 4 x MG 2, MG 5) and a stage-3 pipeline of 4 groups
 SHAPES = [
-    ("conv_pre", 192, 512, 7, 0, 1, "bias_b", 0),
-    ("ups0", 512, 256, 16, 8, 1, "plain", 0),
-    ("ups4", 32, 16, 2, 2, 1, "plain", 0),
-    ("s0_c1_k11_d5", 256, 256, 11, 0, 5, "plain", 0),
-    ("s0_c2_res", 256, 256, 3, 0, 1, "residual", 0),
-    ("s0_c2_acc", 256, 256, 7, 0, 1, "accumulate", 0),
-    ("s1_c1_k7_d3_st4", 128, 128, 7, 0, 3, "plain", 4),
-    ("s2_c2_res_st1", 64, 64, 11, 0, 1, "residual", 1),
-    ("s4_resident_acc", 16, 16, 11, 0, 1, "accumulate", 0),
-    ("s4_resident_c1_d5", 16, 16, 3, 0, 5, "plain", 0),
+    ("conv_pre", 192, 512, 7, 0, 1, "bias_b", 0, 300, None),
+    ("ups0", 512, 256, 16, 8, 1, "plain", 0, 300, None),
+    ("ups4", 32, 16, 2, 2, 1, "plain", 0, 300, None),
+    ("s0_c1_k11_d5", 256, 256, 11, 0, 5, "plain", 0, 300, None),
+    ("s0_c2_res", 256, 256, 3, 0, 1, "residual", 0, 300, None),
+    ("s0_c2_acc", 256, 256, 7, 0, 1, "accumulate", 0, 300, None),
+    ("s3_c1_k7_d3_st4", 32, 32, 7, 0, 3, "plain", 4, 600, (4, 1)),
+    ("s2_c2_res_st1", 64, 64, 11, 0, 1, "residual", 1, 300, None),
+    ("s4_resident_acc", 16, 16, 11, 0, 1, "accumulate", 0, 300, None),
+    ("s4_resident_c1_d5", 16, 16, 3, 0, 5, "plain", 0, 300, None),
+    ("s4_c2_res_ng4_mg2", 16, 16, 3, 0, 1, "residual", 8, 1500, (4, 2)),
+    ("s4_c2_acc_mg5", 16, 16, 11, 0, 1, "accumulate", 5, 1500, (1, 5)),
 ]
-T_IN = 300  # M rows of the launch (input rows of a ConvTranspose): crosses 128-row tiles
 
 
 def _windows(T):
@@ -38,9 +40,9 @@ def _bits(a):
 
 @pytest.mark.parametrize("shape", SHAPES, ids=[s[0] for s in SHAPES])
 def test_g2_window_bitwise(shape):
-    name, Cin, Cout, K, u, dil, mode, st = shape
+    name, Cin, Cout, K, u, dil, mode, st, T, expect = shape  # T: M rows of the launch (input rows of a ConvTranspose)
     rng = np.random.default_rng(zlib.crc32(name.encode()))
-    B, T = 2, T_IN
+    B = 2
     To = T * (u or 1)
     pl, pr = g2_pads()
     w = (rng.standard_normal((Cin, Cout, K) if u else (Cout, Cin, K)) / np.sqrt(Cin * K)).astype(np.float32)
@@ -62,8 +64,9 @@ def test_g2_window_bitwise(shape):
     args = g2_args(**kw)
     # initial output: old values where a running sum accumulates, a NaN canary elsewhere; halo rows hold a distinct canary
     y0 = to_h8(rng.standard_normal((B, Cout, To)).astype(np.float32), halo=7.0) if mode == "accumulate" else to_h8(np.full((B, Cout, To), np.nan, np.float32), halo=7.0)
-    yf, _, gf, ef = g2_conv_window(args, 0, -1, y0)
+    yf, pf, gf, ef = g2_conv_window(args, 0, -1, y0)
     assert gf and ef == 0
+    assert expect is None or (pf.NG, pf.MG) == expect, (name, str(pf))
     for a, b in _windows(T):
         yw, plan, g, e = g2_conv_window(args, a * (u or 1), b * (u or 1), y0)
         assert g and e == 0, (a, b)

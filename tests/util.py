@@ -1,9 +1,10 @@
-"""Shared helpers for the parity tests (golden loading, synthetic model/case regeneration)."""
+"""Shared helpers for the parity tests (golden loading, synthetic model/case regeneration, the kernel tests' error report)."""
 import ast
 import functools
 import os
 
 import numpy as np
+import pytest
 import torch
 
 from bert_vits2_b200 import synth
@@ -37,3 +38,15 @@ def case_inputs(meta):
 
 def rms(a, b):
     return float((a.double() - b.double()).pow(2).mean().sqrt())
+
+
+def report(cid, plan, err, tol, mag, ok_mask, coords):
+    """prints the case line (plan, worst err/mag) and fails with the location and plan of the worst element"""
+    ratio = np.where(ok_mask, err / np.maximum(tol, 1e-30), 0.0)
+    bad = ok_mask & ~(err <= tol)
+    emag = float(np.max(np.where(ok_mask & (mag > 0), err / np.maximum(mag, 1e-30), 0.0))) if ok_mask.any() else 0.0
+    print(f"\n  {cid}: {plan} | worst err/mag {emag:.2e}, worst err/tol {float(ratio.max()) if ratio.size else 0.0:.3f}")
+    if bad.any():
+        idx = np.unravel_index(np.argmax(ratio), ratio.shape)
+        pytest.fail(f"{cid}: {int(bad.sum())} element(s) out of bound; worst at {coords}={tuple(int(i) for i in idx)}: "
+                    f"err {float(err[idx]):.3e} > tol {float(tol[idx]):.3e} (mag {float(mag[idx]):.3e}); plan {plan}")
