@@ -1,4 +1,5 @@
-// Hopper tensor-core (wgmma) implicit-GEMM Conv1d on the c4 activation layout, fp32 accumulators in a shared-memory image.
+// Hopper tensor-core (wgmma) implicit-GEMM Conv1d on the c4 activation layout, fp32 accumulators in wgmma registers (one-tile kernel)
+// or in a shared-memory image (persistent kernels).
 // Replaces the 90 dilated MRF convolutions of the HiFi-GAN Generator (reference modules.py:296-309 via
 // models.py:546-552) = 96 % of the MACs of SynthesizerTrn.infer, the ups (models.py:543-545) and the flow convs.
 //
@@ -17,8 +18,8 @@
 //            11-bit significand as TF32 (identical rounding error), twice the tensor-pipe rate, half the shared-memory
 //            operand bytes per MMA and half the L2->SM weight traffic.  Out-of-range values saturate (cvt.rn.satfinite) instead of becoming inf.
 //
-// Warp roles: warp 0 = TMA producer (cp.async.bulk, mbarrier complete_tx), one warpgroup at the end of the block = wgmma
-// issuer, 4 warps = operand prologue (leaky-relu + operand conversion in smem, zero fill of the conv padding
+// Warp roles: warp 0 = TMA producer (cp.async.bulk, mbarrier complete_tx), one warpgroup (persistent kernels) or two (one-tile
+// kernel, 64 rows each) at the end of the block = wgmma issuers, 4 warps = operand prologue (leaky-relu + operand conversion in smem, zero fill of the conv padding
 // rows, fence.proxy.async), 4 warps (the same ones in the one-tile kernel) = epilogue (accumulator init with
 // bias/residual, tail -> scale/mask -> coalesced 16-byte stores, one thread per row of the accumulator image), +1 weight-producer warp.
 #pragma once
@@ -183,7 +184,8 @@ __device__ int* g_tc_err_flag = nullptr;
 namespace tc {
 // Accumulators live in shared memory, in front of every tensor-core kernel's own buffers: an fp32 image [column][ACC_TS rows] of the
 // 128-row tile, addressed like a tensor-memory column/lane pair (taddr = row << 16 | column; the kernels' accumulator base is 0).
-// The MMA warpgroup streams one 64-row x <= 64-column slice of it through registers per weight stage (wg_mma); the epilogue threads
+// The persistent kernels' MMA warpgroup streams one 64-row x <= 64-column slice of it through registers per weight stage (wg_mma); the
+// one-tile kernel's MMA warpgroups read it once before their first MMA and write it once after their last (tc_issuer); the epilogue threads
 // own one row each and read / write whole runs of columns.  ACC_TS = 132: the stride keeps both access patterns free of bank
 // conflicts (a warp's wgmma fragment touches rows r..r+7 of columns c, c+2, c+4, c+6: banks 8k + r).
 constexpr uint32_t ACC_TS = 132;
@@ -241,10 +243,10 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
                  : "=r"(done) : "r"(bar), "r"(parity), "r"(1000000u) : "memory");
     if (!done) mbar_wait_slow(bar, parity);
 }
-// Bounded wait for the MMA warpgroups and the weight producers, written as ONE asm block (no C++ control flow on a per-thread
-// result, no call): a call inside the MMA loop would make ptxas serialise the wgmma pipeline across it (C7510) and demote the
-// loop's descriptor state from uniform registers.  Same timeout protocol as mbar_wait_slow (error flags raised, wait abandoned),
-// minus the printf.
+// Bounded wait written as ONE asm block (no C++ control flow on a per-thread result, no call), used by every role of the wgmma
+// kernels: a call anywhere in a kernel that issues wgmma makes ptxas serialise its wgmma pipeline (C7510), and a call inside the
+// MMA loop also demotes the loop's descriptor state from uniform registers.  Same timeout protocol as mbar_wait_slow (error
+// flags raised, wait abandoned), minus the printf.
 __device__ __forceinline__ void mbar_wait_u(uint32_t bar, uint32_t parity) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t.reg .u32 n, e;\n\t.reg .u64 t0, t1;\n\t"
@@ -593,22 +595,131 @@ __device__ __forceinline__ void xform16_stage(const float4* S, uint4* O, int ncg
         }
     }
 }
+
+// Arrive on an mbarrier from thread 0 of the warpgroup if bar != 0 (bar = 0: nothing to release).  One asm block: a C++ branch here
+// would make ptxas serialise the wgmma pipeline across it.
+__device__ __forceinline__ void wg_release(uint32_t bar) {
+    asm volatile("{\n\t.reg .pred p, e;\n\t.reg .u32 t;\n\tmov.u32 t, %%tid.x;\n\tand.b32 t, t, 127;\n\tsetp.eq.u32 e, t, 0;\n\t"
+                 "setp.ne.and.u32 p, %0, 0, e;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}" ::"r"(bar) : "memory");
+}
+
+// One k-step of a 64-row x NT-column fragment, issued as the 64 / 32 / 16-column slices wg_mma cuts the same N tile into (B advanced
+// by the slice's first column: 8 columns per 128-byte SBO stride = one 16-byte unit per column).
+template <int F16, int NT>
+__device__ __forceinline__ void wg_mma_nt(float* d, uint64_t a, uint64_t b) {
+    if constexpr (NT >= 64) { Wgmma<F16, 64>::mma(d, a, b); wg_mma_nt<F16, NT - 64>(d + 32, a, b + 64); }
+    else if constexpr (NT >= 32) { Wgmma<F16, 32>::mma(d, a, b); wg_mma_nt<F16, NT - 32>(d + 16, a, b + 32); }
+    else if constexpr (NT >= 16) Wgmma<F16, 16>::mma(d, a, b);
+}
 }  // namespace tc
 
+// State the one-tile kernel's MMA issuer carries through its loops (all warpgroup-uniform except img, the thread's own fragment rows).
+// Descriptors are kept as (constant high word, 32-bit low word), as in tc_gen.cuh.
+struct TcIssue {
+    uint32_t bar_ar, bar_ae, bar_wf, bar_we, bar_acc;     // first barrier of each group
+    uint32_t a_lo_base, w_lo_base, a_stage16, w_stage16;  // descriptor low words of ring slot 0 (A: this warpgroup's 64 rows), slot strides
+    uint32_t a_kstep, b_kstep, dil, nas, nws;
+    int nchunks, K;
+    uint64_t hi;
+    float* img;  // accumulator image at (row of this thread's first fragment row, column 0)
+};
+
+// The issuer of one MMA warpgroup of k_tc_conv1d: 64 rows x NT columns of fp32 accumulators in registers (indexed by compile-time
+// constants only), loaded once from the image the epilogue warps initialised (bias, residual, old output) and written back once for
+// the tail.  Per output the fp32 sequence is the init value, then chunk c, tap j, k-step: the order of the image round trip it replaces.
+// Each stage's MMAs are one wgmma group; once the previous group has completed (wait_group 1) its ring slots are released while the
+// current one runs.
+template <int F16, int NT, int NK>
+__device__ __forceinline__ void tc_issuer(const TcIssue& q) {
+    using namespace tc;
+    float acc[NT / 2];
+    const int cq = 2 * (threadIdx.x & 3);
+#pragma unroll
+    for (int i = 0; i < NT / 8; i++) {
+        const float* s = q.img + (size_t)(8 * i + cq) * ACC_TS;
+        acc[4 * i] = s[0]; acc[4 * i + 1] = s[ACC_TS]; acc[4 * i + 2] = s[8]; acc[4 * i + 3] = s[ACC_TS + 8];
+    }
+    uint32_t sa = 0, aph = 0, a_cur = q.a_lo_base;  // activation ring slot, parity, descriptor low word of the slot
+    uint32_t sw = 0, wph = 0, w_cur = q.w_lo_base;  // weight ring
+    uint32_t rel_w = 0, rel_a = 0;                  // slots the previous stage read: released once its MMAs have completed
+    for (int c = 0; c < q.nchunks; c++) {
+        mbar_wait_u(q.bar_ar + 8u * sa, aph);
+        uint32_t a_tap = a_cur;
+        for (int j = 0; j < q.K; j++, a_tap += q.dil) {
+            mbar_wait_u(q.bar_wf + 8u * sw, wph);
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < NK; kk++)
+                wg_mma_nt<F16, NT>(acc, q.hi | (a_tap + (uint32_t)kk * q.a_kstep), q.hi | (w_cur + (uint32_t)kk * q.b_kstep));
+            wgmma_commit();
+            wgmma_wait1();
+            wg_release(rel_w);
+            wg_release(rel_a);
+            rel_w = q.bar_we + 8u * sw;
+            rel_a = j == q.K - 1 ? q.bar_ae + 8u * sa : 0u;
+            w_cur += q.w_stage16;
+            if (++sw == q.nws) { sw = 0; wph ^= 1u; w_cur = q.w_lo_base; }
+        }
+        a_cur += q.a_stage16;
+        if (++sa == q.nas) { sa = 0; aph ^= 1u; a_cur = q.a_lo_base; }
+    }
+    wgmma_wait0();
+    wg_release(rel_w);
+    wg_release(rel_a);
+#pragma unroll
+    for (int i = 0; i < NT / 8; i++) {
+        float* d = q.img + (size_t)(8 * i + cq) * ACC_TS;
+        d[0] = acc[4 * i]; d[ACC_TS] = acc[4 * i + 1]; d[8] = acc[4 * i + 2]; d[ACC_TS + 8] = acc[4 * i + 3];
+    }
+    mbar_arrive(q.bar_acc);
+}
+// (N tile, k-steps per stage) dispatch as a tree of two-way branches (a switch would become a jump table: see tc_gen.cuh); the k-steps
+// of a stage are a compile-time count because a runtime k-step loop makes ptxas insert warpgroup.arrive around its MMAs (C7519).
+// tc_conv_plan admits these N tiles and K chunks.
+template <int F16, int NK>
+__device__ __forceinline__ void tc_issuer_nt(const TcIssue& q, int nt) {
+    if (nt <= 48) {
+        if (nt <= 16) tc_issuer<F16, 16, NK>(q);
+        else if (nt <= 32) tc_issuer<F16, 32, NK>(q);
+        else tc_issuer<F16, 48, NK>(q);
+    } else if (nt <= 96) {
+        if (nt <= 64) tc_issuer<F16, 64, NK>(q);
+        else tc_issuer<F16, 96, NK>(q);
+    } else {
+        if (nt <= 128) tc_issuer<F16, 128, NK>(q);
+        else tc_issuer<F16, 192, NK>(q);
+    }
+}
+template <int F16>
+__device__ __forceinline__ void tc_issuer_nk(const TcIssue& q, int nt, int nk) {
+    if (nk <= 2) {
+        if (nk == 1) tc_issuer_nt<F16, 1>(q, nt);
+        else tc_issuer_nt<F16, 2>(q, nt);
+    } else {
+        if (F16 || nk == 4) tc_issuer_nt<F16, 4>(q, nt);
+        else tc_issuer_nt<F16, 8>(q, nt);
+    }
+}
+inline bool tc_one_tile_nt(int nt) { return nt == 16 || nt == 32 || nt == 48 || nt == 64 || nt == 96 || nt == 128 || nt == 192; }
+// k-steps per weight stage (K chunk / 2 channel groups): 1, 2, 4 (FP16: K chunk <= 64) or 8 (TF32)
+inline bool tc_one_tile_nk(int KC, int f16) { const int nk = KC / (f16 ? 16 : 8); return nk == 1 || nk == 2 || nk == 4 || (!f16 && nk == 8); }
+
 // ------------------------------------------------------------------------------------------------------------
-// One 128*MT-row tile per CTA.  grid: (M blocks of MT*128 time steps, N tiles, B [* heads])
+// One 128-row tile per CTA.  grid: (M blocks of 128 time steps, N tiles, B [* heads])
 //
 // Accumulator-init fusion: before the first MMA the epilogue warps pre-load  bias (+ per-batch bias) (+/- residual)
 // (+ previous output when accumulating)  into the accumulator image while the first TMA loads are in
-// flight; every MMA then accumulates, and the tail is only  the accumulator image -> [relu] -> scale/mask -> store.
+// flight; the two MMA warpgroups (64 rows each) load it into their registers, accumulate every stage there and write the result
+// back once; the tail is only  the accumulator image -> [relu] -> scale/mask -> store.
+// 512 threads: warp 0 activation producer, warps 2-5 operand prologue + accumulator init + tail, warp 6 weight producer, warps 8-15
+// the two MMA warpgroups (warps 1 and 7 idle).
 template <int GEN, int F16>
-__global__ void __launch_bounds__(384, 1) k_tc_conv1d(TcParams p) {
+__global__ void __launch_bounds__(512, 1) k_tc_conv1d(TcParams p) {
     using namespace tc;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = smem_raw + acc_img_bytes(p.acc_cols);  // behind the accumulator image
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int MT = p.MT;
-    const int t0 = p.t_begin + blockIdx.x * 128 * MT, n0 = blockIdx.y * p.nt, z = blockIdx.z;
+    const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;  // shfl: warp-uniform for the compiler
+    const int t0 = p.t_begin + blockIdx.x * 128, n0 = blockIdx.y * p.nt, z = blockIdx.z;
     const int zs = p.zsplit > 1 ? p.zsplit : 1;
     const int b = z / zs, hz = z - b * zs;
     const int xb = p.x_batch_z ? z : b, yb = p.y_batch_z ? z : b;
@@ -625,9 +736,10 @@ __global__ void __launch_bounds__(384, 1) k_tc_conv1d(TcParams p) {
               B_INIT = B_ACC + 1, B_RES = B_ACC + 2;
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < NAS; i++) { mbar_init(BAR(B_AFULL + i), 1); mbar_init(BAR(B_AREADY + i), 128); mbar_init(BAR(B_AEMPTY + i), 1); }
-        for (int i = 0; i < p.nws; i++) { mbar_init(BAR(B_WFULL + i), 1); mbar_init(BAR(B_WEMPTY + i), 1); }
-        mbar_init(BAR(B_ACC), 1);
+        // a ring slot is free once both MMA warpgroups released it; the accumulators are back in the image once all 256 MMA threads stored theirs
+        for (int i = 0; i < NAS; i++) { mbar_init(BAR(B_AFULL + i), 1); mbar_init(BAR(B_AREADY + i), 128); mbar_init(BAR(B_AEMPTY + i), 2); }
+        for (int i = 0; i < p.nws; i++) { mbar_init(BAR(B_WFULL + i), 1); mbar_init(BAR(B_WEMPTY + i), 2); }
+        mbar_init(BAR(B_ACC), 256);
         mbar_init(BAR(B_INIT), 128);
         mbar_init(BAR(B_RES), 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -666,7 +778,7 @@ __global__ void __launch_bounds__(384, 1) k_tc_conv1d(TcParams p) {
         for (int c = 0; c < p.nchunks; c++) {
             const int sa = c % NAS;
             if (lane == 0) {
-                mbar_wait(BAR(B_AEMPTY + sa), ((c / NAS) & 1) ^ 1);
+                mbar_wait_u(BAR(B_AEMPTY + sa), ((c / NAS) & 1) ^ 1);
                 mbar_expect_tx(BAR(B_AFULL + sa), row_bytes * ncg_in);
             }
             __syncwarp();
@@ -695,7 +807,7 @@ __global__ void __launch_bounds__(384, 1) k_tc_conv1d(TcParams p) {
             for (int c = 0; c < p.nchunks; c++) {
                 const int sw = c % p.nws;
                 if (lane == 0) {
-                    mbar_wait(BAR(B_WEMPTY + sw), ((c / p.nws) & 1) ^ 1);
+                    mbar_wait_u(BAR(B_WEMPTY + sw), ((c / p.nws) & 1) ^ 1);
                     mbar_expect_tx(BAR(B_WFULL + sw), rb * ncg);
                 }
                 __syncwarp();
@@ -721,45 +833,27 @@ __global__ void __launch_bounds__(384, 1) k_tc_conv1d(TcParams p) {
             }
         }
     } else if (warp >= 8) {
-        {  // the 128 threads of the MMA warpgroup run the issue loop together (wgmma is warpgroup-collective)
-            // ===== MMA issuer: per weight tile, MT x KC/(2G) wgmma (M=128, N=nt), always accumulating.
-            // Descriptors are advanced with 64-bit adds on the (addr >> 4) field: ring slot, parity and addresses are carried
-            // incrementally, so the loop body between two stages is a handful of integer instructions.
-            const uint32_t a_lbo = (uint32_t)R * 16u, b_lbo = (uint32_t)nt * 16u;
-            const uint64_t a_kstep = (uint64_t)(2u * (uint32_t)R), b_kstep = (uint64_t)(2u * (uint32_t)nt);  // two channel groups per MMA
-            const int nk = p.KC / (2 * G);
-            mbar_wait_u(BAR(B_INIT), 0);
-            // ring slot / parity / descriptor state carried incrementally: no runtime division or multiply per stage (see tc_gen.cuh)
-            const uint64_t a_stage16 = (uint64_t)(p.a_stage_bytes >> 4), w_stage16 = (uint64_t)(p.w_stage_bytes >> 4);
-            const uint64_t a_desc_base = make_desc(smem_u32(sA) + p.a_op_off, a_lbo, 128u), b_desc_base = make_desc(smem_u32(sW), b_lbo, 128u);
-            const uint32_t bar_ar = BAR(B_AREADY), bar_ae = BAR(B_AEMPTY), bar_wf = BAR(B_WFULL), bar_we = BAR(B_WEMPTY);
-            const uint32_t nas_u = (uint32_t)NAS, nws_u = (uint32_t)p.nws;
-            uint32_t sa = 0, aph = 0, sw = 0, wph = 0;
-            uint64_t a_cur = a_desc_base, b_cur = b_desc_base;
-            for (int c = 0; c < p.nchunks; c++) {
-                mbar_wait_u(bar_ar + 8u * sa, aph);
-                uint64_t a_tap = a_cur;
-                for (int j = 0; j < p.K; j++, a_tap += (uint64_t)(uint32_t)p.dil) {
-                    mbar_wait_u(bar_wf + 8u * sw, wph);
-                    for (int mt = 0; mt < MT; mt++)
-                        wg_mma<F16>(acc0 + (uint32_t)(mt * nt), a_tap + (uint64_t)(uint32_t)(mt * 128), b_cur, a_kstep, b_kstep, nk, nt, 1u);
-                    wg_commit(bar_we + 8u * sw);
-                    b_cur += w_stage16;
-                    if (++sw == nws_u) { sw = 0; wph ^= 1u; b_cur = b_desc_base; }
-                }
-                wg_commit(bar_ae + 8u * sa);
-                a_cur += a_stage16;
-                if (++sa == nas_u) { sa = 0; aph ^= 1u; a_cur = a_desc_base; }
-            }
-            wg_commit(BAR(B_ACC));
-        }
-    } else if (warp == 1 || warp == 7) {  // idle (the MMA warpgroup starts at a warpgroup boundary)
+        // ===== two MMA warpgroups (warps 8-11: rows 0-63, warps 12-15: rows 64-127 of the tile): all 128 threads of a warpgroup run
+        // the issue loop together (wgmma is warpgroup-collective); per weight stage KC/(2G) k-steps of 64 rows x nt columns each
+        const int wg = (warp - 8) >> 2;
+        TcIssue q;
+        q.bar_ar = BAR(B_AREADY); q.bar_ae = BAR(B_AEMPTY); q.bar_wf = BAR(B_WFULL); q.bar_we = BAR(B_WEMPTY); q.bar_acc = BAR(B_ACC);
+        q.a_lo_base = (((smem_u32(sA) + p.a_op_off) & 0x3ffffu) >> 4) + 64u * (uint32_t)wg | (((uint32_t)R * 16u) >> 4) << 16;  // + 64 rows x 16 B
+        q.w_lo_base = ((smem_u32(sW) & 0x3ffffu) >> 4) | (((uint32_t)nt * 16u) >> 4) << 16;
+        q.a_stage16 = p.a_stage_bytes >> 4; q.w_stage16 = p.w_stage_bytes >> 4;
+        q.a_kstep = 2u * (uint32_t)R; q.b_kstep = 2u * (uint32_t)nt;  // two channel groups per MMA
+        q.dil = (uint32_t)p.dil; q.nas = (uint32_t)NAS; q.nws = (uint32_t)p.nws;
+        q.nchunks = p.nchunks; q.K = p.K;
+        q.hi = (uint64_t)(128u >> 4) << 32;  // SBO = 128 B
+        q.img = acc_ptr(acc0) + 64 * wg + 16 * (warp & 3) + (lane >> 2);
+        mbar_wait_u(BAR(B_INIT), 0);
+        tc_issuer_nk<F16>(q, nt, p.KC / (2 * G));
+    } else if (warp == 1 || warp == 7) {  // idle (the MMA warpgroups start at a warpgroup boundary)
     } else {
         const int tid2 = threadIdx.x - 64;
         const int q = warp & 3;
         // ===== accumulator init (overlaps the first TMA loads)
-        for (int mt = 0; mt < MT; mt++)
-            acc_init_tile<4, GEN>(p, acc0 + ((uint32_t)(q * 32) << 16) + (uint32_t)(mt * nt), b, t0 + mt * 128 + q * 32 + lane, n0, nt, yb, cout_off, res_smem);
+        acc_init_tile<4, GEN>(p, acc0 + ((uint32_t)(q * 32) << 16), b, t0 + q * 32 + lane, n0, nt, yb, cout_off, res_smem);
         mbar_arrive(BAR(B_INIT));
         if (bias_only) {  // the init above touched static data only; everything below reads / overwrites tensors of the upstream kernel
             asm volatile("griddepcontrol.wait;" ::: "memory");
@@ -771,7 +865,7 @@ __global__ void __launch_bounds__(384, 1) k_tc_conv1d(TcParams p) {
         const float slope = p.in_slope;
         for (int c = 0; c < p.nchunks; c++) {
             const int sa = c % NAS;
-            mbar_wait(BAR(B_AFULL + sa), (c / NAS) & 1);
+            mbar_wait_u(BAR(B_AFULL + sa), (c / NAS) & 1);
             uint8_t* st = sA + (size_t)sa * p.a_stage_bytes;
             if (F16) {
                 if (!p.in_f16) xform16_stage(reinterpret_cast<const float4*>(st), reinterpret_cast<uint4*>(st + p.a_op_off), p.KC / 8, R, r_lo, r_mask_hi, slope, tid2);
@@ -792,14 +886,13 @@ __global__ void __launch_bounds__(384, 1) k_tc_conv1d(TcParams p) {
             mbar_arrive(BAR(B_AREADY + sa));
         }
         // ===== tail
-        mbar_wait(BAR(B_ACC), 0);
+        mbar_wait_u(BAR(B_ACC), 0);
         if (GEN && p.ln_gamma) {
             const float4* rs = nullptr;
-            if (res_smem) { mbar_wait(BAR(B_RES), 0); rs = reinterpret_cast<const float4*>(smem + p.res_soff) + (q * 32 + lane); }
+            if (res_smem) { mbar_wait_u(BAR(B_RES), 0); rs = reinterpret_cast<const float4*>(smem + p.res_soff) + (q * 32 + lane); }
             acc_tail_ln(p, acc0 + ((uint32_t)(q * 32) << 16), b, t0 + q * 32 + lane, nt, len, rs);
         } else {
-            for (int mt = 0; mt < MT; mt++)
-                acc_tail_tile<4, GEN>(p, acc0 + ((uint32_t)(q * 32) << 16) + (uint32_t)(mt * nt), b, t0 + mt * 128 + q * 32 + lane, n0, nt, len, yb, cout_off);
+            acc_tail_tile<4, GEN>(p, acc0 + ((uint32_t)(q * 32) << 16), b, t0 + q * 32 + lane, n0, nt, len, yb, cout_off);
         }
     }
     __syncthreads();
@@ -854,7 +947,7 @@ __global__ void __launch_bounds__(512, 1) k_tc_conv1d_persist(TcParams p, int mt
             const uint32_t row_bytes = (uint32_t)(r_hi - r_lo) * 16u;
             const int sa = i % NAS;
             if (lane == 0) {
-                mbar_wait(BAR(B_AEMPTY + sa), ((i / NAS) & 1) ^ 1);
+                mbar_wait_u(BAR(B_AEMPTY + sa), ((i / NAS) & 1) ^ 1);
                 mbar_expect_tx(BAR(B_AFULL + sa), row_bytes * ncg_in);
             }
             __syncwarp();
@@ -899,7 +992,7 @@ __global__ void __launch_bounds__(512, 1) k_tc_conv1d_persist(TcParams p, int mt
             const int r_lo = max(0, p.pad - t0), r_hi = min(R, p.T - (t0 - p.pad));
             const int r_mask_hi = p.in_mask ? min(r_hi, len - (t0 - p.pad)) : r_hi;
             const int sa = i % NAS;
-            mbar_wait(BAR(B_AFULL + sa), (i / NAS) & 1);
+            mbar_wait_u(BAR(B_AFULL + sa), (i / NAS) & 1);
             uint8_t* st = sA + (size_t)sa * p.a_stage_bytes;
             if (F16) xform16_stage(reinterpret_cast<const float4*>(st), reinterpret_cast<uint4*>(st + p.a_op_off), ncg, R, r_lo, r_mask_hi, slope, tid2);
             else xform_stage(reinterpret_cast<float4*>(st), ncg, R, r_lo, r_mask_hi, slope, tid2);
@@ -921,7 +1014,7 @@ __global__ void __launch_bounds__(512, 1) k_tc_conv1d_persist(TcParams p, int mt
             if (i + 1 < n_mine) init_tile(i + 1);
             const int tile = blockIdx.x + i * gridDim.x, b = tile / mtiles, t0 = p.t_begin + (tile - b * mtiles) * 128;
             const int len = p.lens ? p.lens[b] : p.T;
-            mbar_wait(BAR(B_ACC + (i & 1)), (i >> 1) & 1);
+            mbar_wait_u(BAR(B_ACC + (i & 1)), (i >> 1) & 1);
             acc_tail_tile<4, GEN>(p, acc0 + ((uint32_t)(q * 32) << 16) + (uint32_t)((i & 1) * nt), b, t0 + q * 32 + lane, 0, nt, len);
         }
     }
@@ -985,7 +1078,7 @@ __global__ void __launch_bounds__(512, 1) k_tc_conv1d_pstream(TcParams p, int mt
             const uint32_t row_bytes = (uint32_t)(r_hi - r_lo) * 16u;
             const int sa = s_ % NAS;
             if (lane == 0) {
-                mbar_wait(BAR(B_AEMPTY + sa), ((s_ / NAS) & 1) ^ 1);
+                mbar_wait_u(BAR(B_AEMPTY + sa), ((s_ / NAS) & 1) ^ 1);
                 mbar_expect_tx(BAR(B_AFULL + sa), row_bytes * ncg_in);
             }
             __syncwarp();
@@ -1067,7 +1160,7 @@ __global__ void __launch_bounds__(512, 1) k_tc_conv1d_pstream(TcParams p, int mt
             const int r_lo = max(0, p.pad - t0), r_hi = min(R, p.T - (t0 - p.pad));
             const int r_mask_hi = p.in_mask ? min(r_hi, len - (t0 - p.pad)) : r_hi;
             const int sa = s_ % NAS;
-            mbar_wait(BAR(B_AFULL + sa), (s_ / NAS) & 1);
+            mbar_wait_u(BAR(B_AFULL + sa), (s_ / NAS) & 1);
             uint8_t* st = sA + (size_t)sa * p.a_stage_bytes;
             if (F16) xform16_stage(reinterpret_cast<const float4*>(st), reinterpret_cast<uint4*>(st + p.a_op_off), p.KC / 8, R, r_lo, r_mask_hi, slope, tid2);
             else xform_stage(reinterpret_cast<float4*>(st), p.KC / 4, R, r_lo, r_mask_hi, slope, tid2);
@@ -1094,7 +1187,7 @@ __global__ void __launch_bounds__(512, 1) k_tc_conv1d_pstream(TcParams p, int mt
             decode(i, b, t0, ntile);
             const int n0 = ntile * nt;
             const int len = p.lens ? p.lens[b] : p.T;
-            mbar_wait(BAR(B_ACC + (i & 1)), (i >> 1) & 1);
+            mbar_wait_u(BAR(B_ACC + (i & 1)), (i >> 1) & 1);
             for (int mt = 0; mt < MT; mt++)
                 acc_tail_tile<8, GEN>(p, acc0 + ((uint32_t)(q * 32) << 16) + (uint32_t)(((i & 1) * MT + mt) * nt), b, t0 + mt * 128 + q * 32 + lane, n0, nt, len);
         }
@@ -1233,11 +1326,10 @@ inline TcConvPlan tc_conv_plan(const TcConvW& w, const float* bias, const Act& x
         pl.mtiles = mtiles; pl.ntiles = ntiles; pl.total = total;
         return pl;
     }
-    // ---- one tile per CTA.  Shared memory per CTA is capped (~48 KB) when there are more CTAs than SMs so that several
-    // CTAs co-reside: one CTA's accumulator init / tail overlaps the other's MMA main loop
-    uint32_t budget = (nctas > num_sms && nt <= 128) ? 48 * 1024 : 200 * 1024;
-    if (nt > 128 && 2 * nctas > num_sms && 2ull * p.a_stage_bytes + 2ull * p.w_stage_bytes + 2048 <= 112 * 1024)
-        budget = 112 * 1024;  // wide layer launched on three streams at once (MRF resblock chains): let two CTAs share an SM
+    // ---- one tile per CTA.  512 threads holding up to 96 fp32 accumulators each: one CTA per SM, so the rings take what the SM has.
+    BV2_CHECK(tc_one_tile_nt(nt) && tc_one_tile_nk(p.KC, F16), "tc_conv1d: no one-tile MMA issuer for N tile " + std::to_string(nt) + " / K chunk " +
+              std::to_string(p.KC) + " (N tile 16, 32, 48, 64, 96, 128 or 192; K chunk of 1, 2, 4 or (TF32) 8 k-steps)");
+    uint32_t budget = 200 * 1024;
     // LayerNorm tail with a residual, at most one CTA per SM (small batches: the launch is a latency chain, not a throughput problem):
     // the residual tile is staged in shared memory by TMA (nt/4 channel groups x 128 rows x 16 B) instead of being pre-loaded into the
     // accumulator; the rings shrink to make room (the weight ring never needs more stages than the conv has)
@@ -1258,7 +1350,7 @@ inline TcConvPlan tc_conv_plan(const TcConvW& w, const float* bias, const Act& x
     if (res_smem) { smem = (smem + 15) & ~(size_t)15; p.res_soff = (uint32_t)(smem - img); smem += res_bytes; }  // offset from the kernel's `smem` (behind the image)
     BV2_CHECK(smem <= 227 * 1024, "tc_conv1d shared memory");
     pl.kind = TC_ONE_TILE; pl.res_smem = res_smem ? 1 : 0; pl.nas = p.nas; pl.nws = p.nws; pl.smem = smem;
-    pl.grid = dim3(cdiv(wrows, 128), ntiles, p.B); pl.block = dim3(384);
+    pl.grid = dim3(cdiv(wrows, 128), ntiles, p.B); pl.block = dim3(512);
     pl.mtiles = cdiv(wrows, 128); pl.ntiles = ntiles; pl.total = pl.mtiles * ntiles * p.B;
     return pl;
 }
@@ -1285,6 +1377,7 @@ inline void tc_launch_simple(TcParams& p, int ntiles, int zdim, cudaStream_t st)
     p.MT = 1; p.R = 128 + halo; p.pad = (p.K - 1) / 2 * p.dil;
     p.a_stage_bytes = (uint32_t)(p.KC * p.R * 4); p.a_op_off = 0;
     p.w_stage_bytes = (uint32_t)(p.KC * p.nt * 4);
+    BV2_CHECK(tc_one_tile_nt(p.nt) && tc_one_tile_nk(p.KC, 0), "tc gemm N tile / K chunk");
     const long long nctas = (long long)cdiv(p.T, 128) * ntiles * zdim;
     const uint32_t img = tc::acc_img_bytes((uint32_t)p.nt);
     const uint32_t budget = std::min<uint32_t>(nctas > 132 ? 100 * 1024 : 200 * 1024, 220 * 1024 - img);
@@ -1297,7 +1390,7 @@ inline void tc_launch_simple(TcParams& p, int ntiles, int zdim, cudaStream_t st)
     const size_t smem = img + (size_t)p.nas * p.a_stage_bytes + (size_t)p.nws * p.w_stage_bytes + (size_t)(3 * p.nas + 2 * p.nws + 3) * 8 + 16;
     BV2_CHECK(smem <= 227 * 1024, "tc gemm shared memory");
     dim3 grid(cdiv(p.T, 128), ntiles, zdim);
-    launch_pdl(k_tc_conv1d<0, 0>, grid, dim3(384), smem, st, p);
+    launch_pdl(k_tc_conv1d<0, 0>, grid, dim3(512), smem, st, p);
 }
 
 // S[z][keys][queries] (c4 over keys) = Q . K^T for every (batch, head): qkv c4 [B][3H/4][T][4], q pre-scaled.

@@ -79,13 +79,6 @@ struct G2Issue {
     float* img;                                            // accumulator image at (row of this thread's first fragment row, column 0)
 };
 
-// Arrive on an mbarrier from thread 0 of the warpgroup if bar != 0 (bar = 0: nothing to release).  One asm block: a C++ branch here
-// would make ptxas serialise the wgmma pipeline across it.
-__device__ __forceinline__ void g2_release(uint32_t bar) {
-    asm volatile("{\n\t.reg .pred p, e;\n\t.reg .u32 t;\n\tmov.u32 t, %%tid.x;\n\tand.b32 t, t, 127;\n\tsetp.eq.u32 e, t, 0;\n\t"
-                 "setp.ne.and.u32 p, %0, 0, e;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}" ::"r"(bar) : "memory");
-}
-
 // The issuer's loop nest for one (NK, MG, NT) instantiation, run by each of the two MMA warpgroups on its 64 rows of every m-tile.
 // A group's accumulators stay in registers (MG x NT/2 fp32 per thread, indexed by compile-time constants only) from the bias to the
 // last k-step; the accumulator image is written once per group, for the epilogue.  Per output the fp32 sequence is bias, then chunk c,
@@ -125,8 +118,8 @@ __device__ __forceinline__ void g2_issuer(const G2Issue& q) {
                         Wgmma<1, NT>::mma(acc[mt], q.hi | (a_tap + (uint32_t)(mt * 128) + (uint32_t)kk * q.a_kstep), q.hi | (w_cur + (uint32_t)kk * q.b_kstep));
                 wgmma_commit();
                 wgmma_wait1();
-                g2_release(rel_w);
-                g2_release(rel_a);
+                wg_release(rel_w);
+                wg_release(rel_a);
                 rel_w = q.streamed ? q.bar_we + 8u * sw : 0u;
                 rel_a = j == q.K - 1 ? q.bar_ae + 8u * sa : 0u;
                 w_cur += q.w_stage16;
@@ -136,8 +129,8 @@ __device__ __forceinline__ void g2_issuer(const G2Issue& q) {
             if (++sa == q.nas) { sa = 0; aph ^= 1u; a_cur = q.a_lo_base; }
         }
         wgmma_wait0();
-        g2_release(rel_w);
-        g2_release(rel_a);
+        wg_release(rel_w);
+        wg_release(rel_a);
         // hand-off: the group's columns of the image (same fragment-to-image map as tc::wg_slice), then one arrival per thread
         float* im = q.img + (size_t)(g * MG * NT + cq) * ACC_TS;
 #pragma unroll
