@@ -22,6 +22,9 @@ STREAM_HARNESS_PATH = os.path.join(HERE, "libbv2_stream_harness.so")
 # bounded-stream harness (tests/cuda/stream_bounded_harness.cu): the resident-range planner and launches, on top of the kernel harness
 BOUNDED_HARNESS_SOURCE = os.path.join(ROOT, "tests", "cuda", "stream_bounded_harness.cu")
 BOUNDED_HARNESS_PATH = os.path.join(HERE, "libbv2_stream_bounded_harness.so")
+# ragged-batch harness (tests/cuda/ragged_harness.cu): a k_g2_conv launch whose items stop at their own lengths, on top of the kernel harness
+RAGGED_HARNESS_SOURCE = os.path.join(ROOT, "tests", "cuda", "ragged_harness.cu")
+RAGGED_HARNESS_PATH = os.path.join(HERE, "libbv2_ragged_harness.so")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
 MAX_UPS, MAX_RK, MAX_DIL = 8, 4, 4
@@ -54,6 +57,8 @@ SYMBOLS = {
                                   C.c_float, C.c_float, F32P, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
     "bv2_infer_finish": (C.c_int, [P, F32P, C.c_int64, C.c_float, C.c_int32, F32P, F32P, F32P, F32P, F32P, F32P, F32P, C.c_void_p]),
     "bv2_infer_finish_pcm16": (C.c_int, [P, F32P, C.c_int64, C.c_float, C.c_int32, C.c_void_p, F32P, F32P, F32P, F32P, F32P, F32P, C.c_void_p]),
+    "bv2_infer_finish_ragged": (C.c_int, [P, F32P, C.c_int64, C.c_float, C.c_int32, F32P, C.c_void_p, F32P, F32P, F32P, F32P, F32P, F32P,
+                                          C.c_void_p]),
     "bv2_infer_finish_stream": (C.c_int, [P, F32P, C.c_int64, C.c_float, C.c_int32, F32P, F32P, F32P, F32P, F32P, F32P, F32P, C.c_void_p]),
     "bv2_stream_advance": (C.c_int, [P, C.c_int32, C.c_void_p, C.POINTER(C.c_int64)]),
     "bv2_infer_finish_stream_bounded": (C.c_int, [P, F32P, C.c_int64, C.c_float, C.c_int32, C.c_int32, F32P, F32P, F32P, F32P, F32P, F32P, F32P,
@@ -67,6 +72,7 @@ SYMBOLS = {
     "bv2_duration": (C.c_int, [P, C.c_int, C.c_int, F32P, I64P, I64P, F32P, C.c_float, F32P, F32P, C.c_void_p]),
     "bv2_flow_reverse": (C.c_int, [P, C.c_int, C.c_int, F32P, I64P, I64P, F32P, C.c_void_p]),
     "bv2_generator": (C.c_int, [P, C.c_int, C.c_int, F32P, F32P, F32P, C.c_void_p]),
+    "bv2_generator_ragged": (C.c_int, [P, C.c_int, C.c_int, F32P, F32P, I64P, F32P, C.c_void_p]),
     "bv2_debug_read": (C.c_int64, [P, C.c_char_p, C.c_void_p, C.c_int64]),
     "bv2_set_profiling": (C.c_int, [P, C.c_int]),
     "bv2_stage_ms": (C.c_float, [P, C.c_char_p]),
@@ -111,15 +117,17 @@ def build(force: bool = False, verbose: bool = False) -> str:
         return LIB_PATH
 
 
-def _harness(stream: bool, bounded: bool):
+def _harness(stream: bool, bounded: bool, ragged: bool = False):
     """(source, library) of a test harness"""
+    if ragged:
+        return RAGGED_HARNESS_SOURCE, RAGGED_HARNESS_PATH
     if bounded:
         return BOUNDED_HARNESS_SOURCE, BOUNDED_HARNESS_PATH
     return (STREAM_HARNESS_SOURCE, STREAM_HARNESS_PATH) if stream else (HARNESS_SOURCE, HARNESS_PATH)
 
 
-def harness_needs_build(stream: bool = False, bounded: bool = False) -> bool:
-    src, path = _harness(stream, bounded)
+def harness_needs_build(stream: bool = False, bounded: bool = False, ragged: bool = False) -> bool:
+    src, path = _harness(stream, bounded, ragged)
     if not os.path.isfile(path):
         return True
     t = os.path.getmtime(path)
@@ -127,12 +135,12 @@ def harness_needs_build(stream: bool = False, bounded: bool = False) -> bool:
     return any(os.path.getmtime(p) > t for p in deps if os.path.isfile(p))
 
 
-def build_harness(force: bool = False, stream: bool = False, bounded: bool = False) -> str:
-    """Compile the kernel test harness (stream=True: the streaming harness, bounded=True: the bounded-stream harness) next to
-    libbv2.so with the product flags."""
-    src, path = _harness(stream, bounded)
+def build_harness(force: bool = False, stream: bool = False, bounded: bool = False, ragged: bool = False) -> str:
+    """Compile the kernel test harness (stream=True: the streaming harness, bounded=True: the bounded-stream harness, ragged=True:
+    the ragged-batch harness) next to libbv2.so with the product flags."""
+    src, path = _harness(stream, bounded, ragged)
     with _lock:
-        if not force and not harness_needs_build(stream, bounded):
+        if not force and not harness_needs_build(stream, bounded, ragged):
             return path
         tmp = path + ".tmp"
         r = subprocess.run(["nvcc"] + NVCC_FLAGS + ["-o", tmp, src], capture_output=True, text=True)

@@ -399,8 +399,9 @@ struct bv2_engine : DeviceWeights {
                        cudaStream_t s);
     void run_dp(Act h, const int* lens, const float* gproj, Act& dp_out, Act xg, Act d1, Act d2, cudaStream_t s);
     void run_flow(Act z, const int* lens, const float* gproj, cudaStream_t s);
-    void run_generator(Act z, const int* lens_or_null, const float* gdec, int g_stride, float* o, cudaStream_t s);
-    void run_generator_g2(Act z, const int* lens_or_null, const float* gdec, int g_stride, float* o, cudaStream_t s);
+    // ragged: batch item b runs at its own length lens[b] (clamped to z.T) instead of z.T: FP16 Generator only, else BV2_ERR_ARG
+    void run_generator(Act z, const int* lens_or_null, const float* gdec, int g_stride, float* o, cudaStream_t s, bool ragged = false);
+    void run_generator_g2(Act z, const int* lens_or_null, const float* gdec, int g_stride, float* o, cudaStream_t s, bool ragged);
     H8 g2_h8(int B, int C, int T, int rows = -1);
     H8 g2_input(Act z, const int* lens_or_null, cudaStream_t s);
     size_t stream_bytes(int B, int Fg, int max_chunk) const;
@@ -409,7 +410,7 @@ struct bv2_engine : DeviceWeights {
     void gen_windows(const GenGraph& g, const std::vector<GenWin>& w, std::vector<Act>& t, bool stream, const int* lens_or_null, const float* gdec,
                      int g_stride, float* o, cudaStream_t s);
     void g2_windows(const GenGraph& g, const std::vector<GenWin>& w, std::vector<H8>& t, bool stream, const float* gdec, int g_stride,
-                    float* o, cudaStream_t s);
+                    float* o, cudaStream_t s, const int* ragged_lens = nullptr);
     int* lens_to_device(const int64_t* x_lengths_dev, int B, Arena& ar, cudaStream_t s);
     // ids inside their tables, 1 <= lengths <= T (the reference raises IndexError / a shape error): device-side check into *err_dev
     void launch_validate(int B, int T, const int64_t* x, const int64_t* tone, const int64_t* lang, const int64_t* sid, const int64_t* lens,
@@ -476,6 +477,11 @@ struct bv2_engine : DeviceWeights {
 __global__ void k_i64_to_i32(const long long* __restrict__ a, int* __restrict__ b, int n) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) b[i] = (int)a[i];
+}
+// lengths clamped to [1, hi] (bv2_generator_ragged: an out-of-range length never becomes an out-of-range row)
+__global__ void k_lengths_clamp(const long long* __restrict__ a, int* __restrict__ b, int n, int hi) {
+    int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) b[i] = (int)max(1ll, min((long long)hi, a[i]));
 }
 __global__ void k_scale_copy(const float* __restrict__ a, float* __restrict__ b, float s, size_t n) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1004,8 +1010,9 @@ void bv2_engine::run_flow(Act z, const int* lens, const float* gproj, cudaStream
 
 // Generator.forward (reference models.py:538-557) + ResBlock1.forward (modules.py:296-309).  The one-shot run is the one-chunk plan of a
 // stream (gen_stream.cuh): every window covers its whole layer.
-void bv2_engine::run_generator(Act z, const int* lens, const float* gdec, int g_stride, float* o, cudaStream_t s) {
-    if (use_g2) { run_generator_g2(z, lens, gdec, g_stride, o, s); return; }
+void bv2_engine::run_generator(Act z, const int* lens, const float* gdec, int g_stride, float* o, cudaStream_t s, bool ragged) {
+    if (use_g2) { run_generator_g2(z, lens, gdec, g_stride, o, s, ragged); return; }
+    if (ragged) throw Error(BV2_ERR_ARG, "a ragged batch needs the FP16 Generator (precision fp16 or fp16g)");
     const GenGraph g = gen_graph(cfg, z.T);
     std::vector<Act> t(g.tensor_len.size());
     t[0] = z;
@@ -1112,11 +1119,14 @@ void bv2_engine::gen_windows(const GenGraph& g, const std::vector<GenWin>& w, st
 // Generator on 16-bit activation tensors (tc_gen.cuh): every tensor between conv_pre and conv_post is an H8 operand image
 // (f16(lrelu_0.1(x)), zero halos); 96 launches of ONE kernel (k_g2_conv) + conv_post.  The one-shot run is the one-chunk plan of a
 // stream (gen_stream.cuh): every window covers its whole layer.
-void bv2_engine::run_generator_g2(Act z, const int* lens, const float* gdec, int g_stride, float* o, cudaStream_t s) {
+// ragged: item b's rows stop at min(lens[b], z.T) frames in every layer, each followed by its own zero halo, so it computes exactly what a
+// run of that item alone at that length computes (same launches, same workspace; samples past its length are 0).
+void bv2_engine::run_generator_g2(Act z, const int* lens, const float* gdec, int g_stride, float* o, cudaStream_t s, bool ragged) {
+    BV2_CHECK(!ragged || lens, "ragged Generator without lengths");
     const GenGraph g = gen_graph(cfg, z.T);
     std::vector<H8> t(g.tensor_len.size());
     t[0] = g2_input(z, lens, s);
-    g2_windows(g, gen_stream_plan(g, z.T, 0, z.T), t, false, gdec, g_stride, o, s);
+    g2_windows(g, gen_stream_plan(g, z.T, 0, z.T), t, false, gdec, g_stride, o, s, ragged ? lens : nullptr);
 }
 
 // rows >= 0: storage for only that many rows (a stream's tensor, H8::base); else the whole tensor
@@ -1200,9 +1210,10 @@ void bv2_engine::g2_stream_prepare(int done, int target, cudaStream_t s) {
 // GenGraph tensor.  stream = false: a one-shot run over whole layers; t holds only the input, and the stage temporaries are
 // bump-allocated per stage and released after the join (the convs of one resblock chain share one temporary and two ping-pong
 // buffers).  stream = true: a chunk of a stream, on tensors that live as long as the stream and hold the rows of gen_stream_rows().
-// Every tensor is addressed by logical row through its base (0 for a whole tensor).
+// Every tensor is addressed by logical row through its base (0 for a whole tensor).  ragged_lens (device, frames per item; null: every
+// item has all g.tensor_len[0] frames): every layer stores item b's rows below its length only, at the layer's rows per frame.
 void bv2_engine::g2_windows(const GenGraph& g, const std::vector<GenWin>& w, std::vector<H8>& t, bool stream, const float* gdec, int g_stride,
-                            float* o, cudaStream_t s) {
+                            float* o, cudaStream_t s, const int* ragged_lens) {
     const int B = t[0].B;
     int li = 0;
     auto conv = [&](const TcConvW& cw, const float* bias, G2Epi e, cudaStream_t sj) {
@@ -1210,6 +1221,7 @@ void bv2_engine::g2_windows(const GenGraph& g, const std::vector<GenWin>& w, std
         const GenWin& wi = w[li++];
         if (wi.t_end <= wi.t_begin) return;
         e.t_begin = wi.t_begin; e.t_end = wi.t_end;
+        if (ragged_lens) { e.lens = ragged_lens; e.lens_scale = l.L_in / g.tensor_len[0]; }  // the M axis is the input's time axis
         if (l.res >= 0) e.res = &t[l.res];
         g2_conv(cw, bias, t[l.in], t[l.out], e, sj, num_sms); launches++;
     };
@@ -1267,7 +1279,9 @@ void bv2_engine::g2_windows(const GenGraph& g, const std::vector<GenWin>& w, std
     const GenWin& wp = w[li];
     if (wp.t_end > wp.t_begin) {
         BV2_CHECK((x.base == 0 || wp.t_begin - 3 >= x.base) && std::min(wp.t_end + 3, x.T + G2_PADR) <= x.lim(), "conv_post input rows not resident");
-        launch_pdl(k_conv_post_tanh_h8<16, 7>, dim3(cdiv(wp.t_end - wp.t_begin, 512), B), dim3(256), 0, s, (const uint4*)x.p, x.Tp, x.base, conv_post_h, o,
+        PostW<16, 7> pw = conv_post_h;
+        if (ragged_lens) { pw.lens = ragged_lens; pw.lens_scale = g.hop; }
+        launch_pdl(ragged_lens ? k_conv_post_tanh_h8<16, 7, true> : k_conv_post_tanh_h8<16, 7>, dim3(cdiv(wp.t_end - wp.t_begin, 512), B), dim3(256), 0, s, (const uint4*)x.p, x.Tp, x.base, pw, o,
                    lp.L_out, wp.t_begin, wp.t_end);
         launches++;
     }
@@ -1501,13 +1515,15 @@ int bv2_infer_begin(bv2_engine* e, int B, int T, const int64_t* x, const int64_t
 }
 
 // open_stream: stop after the flow and open a Generator stream over o instead of running the Generator (bv2_infer_finish_stream)
+// ragged: the Generator runs each utterance at its own length (bv2_infer_finish_ragged)
 static int infer_finish_impl(bv2_engine* e, const float* noise_z, int64_t noise_ld, float noise_scale, int32_t max_len, float* o, int16_t* o16,
                              float* attn, float* y_mask, float* z_out, float* z_p, float* m_p, float* logs_p, void* stream, bool open_stream = false,
-                             int max_chunk = 0) {
+                             int max_chunk = 0, bool ragged = false) {
     BV2_API_BEGIN(e)
     auto& st = e->st;
     BV2_CHECK(st.active, "infer_finish without infer_begin");
     BV2_CHECK(noise_z && (o || o16) && noise_ld >= st.F, "infer_finish args");
+    if (ragged && !e->use_g2) throw Error(BV2_ERR_ARG, "a ragged batch needs the FP16 Generator (precision fp16 or fp16g)");
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const bv2_config& c = e->cfg;
     const int B = st.B, T = st.T, F = st.F, I = c.inter_channels;
@@ -1556,10 +1572,10 @@ static int infer_finish_impl(bv2_engine* e, const float* noise_z, int64_t noise_
         float* wf = e->ws.alloc((size_t)B * L);
         unsigned* peak = reinterpret_cast<unsigned*>(e->ws.alloc(B));
         long long* nval = reinterpret_cast<long long*>(e->ws.alloc(2 * (size_t)B));
-        e->run_generator(zg, st.ylen32, st.gproj + e->goff_dec, e->gproj_n, wf, s);
+        e->run_generator(zg, st.ylen32, st.gproj + e->goff_dec, e->gproj_n, wf, s, ragged);
         e->pcm16(wf, B, L, st.ylen, e->hop, nval, peak, o16, s);
     } else {
-        e->run_generator(zg, st.ylen32, st.gproj + e->goff_dec, e->gproj_n, o, s);
+        e->run_generator(zg, st.ylen32, st.gproj + e->goff_dec, e->gproj_n, o, s, ragged);
     }
     e->stage_end("generator", s);
     st.active = false; st.finished = true;
@@ -1576,6 +1592,12 @@ int bv2_infer_finish_pcm16(bv2_engine* e, const float* noise_z, int64_t noise_ld
                            float* attn, float* y_mask, float* z_out, float* z_p, float* m_p, float* logs_p, void* stream) {
     if (!o16) return BV2_ERR_ARG;
     return infer_finish_impl(e, noise_z, noise_ld, noise_scale, max_len, nullptr, o16, attn, y_mask, z_out, z_p, m_p, logs_p, stream);
+}
+
+int bv2_infer_finish_ragged(bv2_engine* e, const float* noise_z, int64_t noise_ld, float noise_scale, int32_t max_len, float* o, int16_t* o16,
+                            float* attn, float* y_mask, float* z_out, float* z_p, float* m_p, float* logs_p, void* stream) {
+    if (!o == !o16) return BV2_ERR_ARG;  // exactly one output
+    return infer_finish_impl(e, noise_z, noise_ld, noise_scale, max_len, o, o16, attn, y_mask, z_out, z_p, m_p, logs_p, stream, false, 0, true);
 }
 
 int bv2_infer_finish_stream_bounded(bv2_engine* e, const float* noise_z, int64_t noise_ld, float noise_scale, int32_t max_len, int32_t max_chunk_frames,
@@ -1759,24 +1781,41 @@ int bv2_flow_reverse(bv2_engine* e, int B, int F, const float* z_p, const int64_
     BV2_API_END(e)
 }
 
-int bv2_generator(bv2_engine* e, int B, int F, const float* z_in, const float* g, float* o, void* stream) {
+// lengths (device, may be null): a ragged batch, item b at its own length clamped to [1, F]
+static int generator_impl(bv2_engine* e, int B, int F, const float* z_in, const float* g, const int64_t* lengths, float* o, void* stream) {
     BV2_API_BEGIN(e)
     BV2_CHECK(e->finalized, "not finalized");
     BV2_CHECK(B >= 1 && F >= 1 && z_in && g && o, "generator args");
+    if (lengths && !e->use_g2) throw Error(BV2_ERR_ARG, "a ragged batch needs the FP16 Generator (precision fp16 or fp16g)");
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const bv2_config& c = e->cfg;
     const int I = c.inter_channels;
     e->dbg.clear(); e->st.active = false;
     e->ws.ensure(ws_bytes_for(c, B, 1, F)); e->ws_reset();
+    int* lens = nullptr;
+    if (lengths) {
+        lens = reinterpret_cast<int*>(e->ws.alloc(B));
+        k_lengths_clamp<<<cdiv(B, 128), 128, 0, s>>>(reinterpret_cast<const long long*>(lengths), lens, B, F);
+        BV2_CUDA(cudaGetLastError()); e->launches++;
+    }
     float* gp = e->ws.alloc((size_t)B * e->gproj_n);
     e->run_gproj(g, B, gp, s);
     Act z = e->ws.act(B, I, F);
     k_plain_to_c4<<<bv2_engine::grid_tcb(F, I, B), 128, 0, s>>>(z_in, I, (long long)I * F, F, z.p, I, 0, F, nullptr, 1.f);
     BV2_CUDA(cudaGetLastError()); e->launches++;
     e->stage_begin("generator", s);
-    e->run_generator(z, nullptr, gp + e->goff_dec, e->gproj_n, o, s);
+    e->run_generator(z, lens, gp + e->goff_dec, e->gproj_n, o, s, lengths != nullptr);
     e->stage_end("generator", s);
     BV2_API_END(e)
+}
+
+int bv2_generator(bv2_engine* e, int B, int F, const float* z_in, const float* g, float* o, void* stream) {
+    return generator_impl(e, B, F, z_in, g, nullptr, o, stream);
+}
+
+int bv2_generator_ragged(bv2_engine* e, int B, int F, const float* z_in, const float* g, const int64_t* lengths, float* o, void* stream) {
+    if (!lengths) return BV2_ERR_ARG;
+    return generator_impl(e, B, F, z_in, g, lengths, o, stream);
 }
 
 int64_t bv2_debug_read(bv2_engine* e, const char* name, float* host_out, int64_t capacity) {

@@ -56,6 +56,11 @@ struct G2Params {
     int residual, accumulate, ups_u, ups_cout;
     float out_scale;
     int x_lim;  // end of the input rows that may be read: the halo's end T + G2_PADR, or the storage's end if that comes first
+    // ragged batch (null: every item has t_end rows): item b has lens[b] frames, lens_scale M-axis rows per frame at this layer.  Its
+    // rows stop at lim = min(t_end, lens[b] * lens_scale), followed by G2_PADR zero rows, exactly as in a run of that item alone.
+    // lens must be complete before the launch (read ahead of the PDL wait).
+    const int* lens;
+    int lens_scale;
 };
 
 namespace tc {
@@ -162,6 +167,12 @@ __device__ __forceinline__ void g2_issuer_nt(const G2Issue& q, int nt, int MG) {
     else { if (nt == 64) g2_issuer_mg<NK, 64, 1, 2>(q, MG); else g2_issuer<NK, 1, 128>(q); }
 }
 
+// End of batch b's rows on the M axis: t_end, or for a ragged batch (G2Params::lens) the end of b's own rows.
+template <bool RAGGED>
+__device__ __forceinline__ int g2_lim(const G2Params& p, int b) { return RAGGED ? min(p.t_end, p.lens[b] * p.lens_scale) : p.t_end; }
+
+// RAGGED = false is the kernel of a batch without lengths, compiled as if the ragged case did not exist (same registers and code).
+template <bool RAGGED>
 __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
     using namespace tc;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -169,6 +180,8 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;  // shfl: warp-uniform for the compiler
     const int NAS = p.nas, NWS = p.nws, NG = p.NG, MG = p.MG, NCH = p.nchunks, nt = p.nt, R = p.R;
     const int t0 = p.t_begin + blockIdx.x * NG * MG * 128, ntile = blockIdx.y, n0 = ntile * nt, b = blockIdx.z;
+    // a CTA wholly past the end of batch b's rows has nothing to store and no halo to clear (CTA-uniform exit before any barrier)
+    if (RAGGED && t0 >= g2_lim<RAGGED>(p, b)) return;
     uint8_t* sA = smem;
     uint8_t* sW = smem + (size_t)NAS * p.a_stage_bytes;
     const int nwst = p.resident ? NCH * p.K : NWS;  // weight stages held in shared memory
@@ -274,17 +287,21 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
         // ===== zero halo of the OUTPUT tensor (= the conv padding of its consumers), written by its producer: the CTA of the first super-tile
         // clears rows [-G2_PADL, 0) if the window starts at t = 0, the CTA of the last one rows [T_out, T_out + G2_PADR) if the window ends at
         // T_out, for every channel group of batch b (N tile 0 only).  A window inside the tensor leaves the halo rows alone: in a streamed run
-        // they are final rows of earlier windows.
-        const bool lo = blockIdx.x == 0 && p.t_begin == 0, hi = blockIdx.x == gridDim.x - 1 && p.t_end == p.T;
+        // they are final rows of earlier windows.  In a ragged batch the trailing halo of item b follows its own rows: the CTA holding row
+        // lim - 1 clears output rows [lim * u, lim * u + G2_PADR) (with lim == T, the tensor's halo).
+        const int lim = g2_lim<RAGGED>(p, b);
+        const bool lo = blockIdx.x == 0 && p.t_begin == 0;
+        const bool hi = RAGGED ? (lim - 1 - p.t_begin) / (NG * MG * 128) == (int)blockIdx.x && (lim < p.t_end || p.t_end == p.T)
+                               : blockIdx.x == gridDim.x - 1 && p.t_end == p.T;
         if (ntile == 0 && (lo || hi)) {
             asm volatile("griddepcontrol.wait;" ::: "memory");  // the rows may alias a tensor an upstream kernel is still reading
             uint4* yb = p.y + (size_t)b * p.y_cg * p.y_Tp;
-            const int Tout = p.T * (p.ups_u ? p.ups_u : 1);
+            const int hrow = (RAGGED ? lim : p.T) * (p.ups_u ? p.ups_u : 1);
             const uint4 z4 = make_uint4(0u, 0u, 0u, 0u);
             if (lo)
                 for (int i = lane; i < p.y_cg * G2_PADL; i += 32) yb[(size_t)(i / G2_PADL) * p.y_Tp + (i % G2_PADL) - G2_PADL] = z4;
             if (hi)
-                for (int i = lane; i < p.y_cg * G2_PADR; i += 32) yb[(size_t)(i / G2_PADR) * p.y_Tp + Tout + (i % G2_PADR)] = z4;
+                for (int i = lane; i < p.y_cg * G2_PADR; i += 32) yb[(size_t)(i / G2_PADR) * p.y_Tp + hrow + (i % G2_PADR)] = z4;
         }
     } else if (warp >= 4) {
         // ===== epilogue, 8 warps (4-11): row quarter q = warp & 3; the 2 warps of a quarter share the (m-tile, 32-column batch) items
@@ -298,12 +315,13 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
         const int ncb = nt >= 32 ? nt / 32 : 1, cw = nt >= 32 ? 32 : 16;  // column batches per m-tile, columns per batch
         asm volatile("griddepcontrol.wait;" ::: "memory");
         const bool scaled = p.out_scale != 1.f;
+        const int lim = g2_lim<RAGGED>(p, b);
         for (int g = 0; g < NG; g++) {
             mbar_wait_u(BAR(B_ACC + g), 0);
             for (int it = part; it < MG * ncb; it += 2) {
                 const int mt = it / ncb, col0 = (it - mt * ncb) * cw;
                 const int t = t0 + (g * MG + mt) * 128 + q * 32 + lane;
-                const bool ok = t < p.t_end;  // stores, residual reads and running-sum updates stay inside the window
+                const bool ok = t < lim;  // stores, residual reads and running-sum updates stay inside the window (and batch b's rows)
                 uint32_t v[32];
                 if (cw == 32) acc_ld<32>(trow + (uint32_t)((g * MG + mt) * nt + col0), v); else acc_ld<16>(trow + (uint32_t)((g * MG + mt) * nt + col0), v);
                 // residual / running-sum operands are fetched while the accumulator image load is in flight
@@ -378,17 +396,24 @@ __global__ void __launch_bounds__(128) k_c4_to_h8(const float4* __restrict__ x, 
 // unpacked + activated K times and every FMA fetched its weight from shared memory (~40 instructions per 16-byte load, 24 us).  Here a block
 // stages TB + K - 1 rows ONCE as activated fp32 in shared memory (coalesced 16-byte loads, conflict-free stores), the weights ride in the
 // kernel parameters (constant bank: FFMA takes them as an operand), and a thread's inner loop is one conflict-free LDS + one FFMA per tap.
-template <int C, int K> struct PostW { float w[C * K]; };  // [C][K]
+// The kernel-parameter block: weights [C][K], and for a ragged batch (RAGGED = true) each item's frame count and the samples per frame:
+// samples of item b from lens[b] * lens_scale on are stored as 0, and a block wholly past that point computes nothing.
+template <int C, int K> struct PostW { float w[C * K]; const int* lens = nullptr; int lens_scale = 0; };
 // Outputs [t_begin, t_end) of the T samples are stored; staged rows past t_end feed discarded outputs only.  x holds the logical rows
 // from x_base (H8::base; 0 for a whole tensor) to the end of its storage; rows from the halo's end T + G2_PADR on, or from the storage's
 // end if that comes first, are read as zero.
-template <int C, int K>
+template <int C, int K, bool RAGGED = false>
 __global__ void __launch_bounds__(256) k_conv_post_tanh_h8(const uint4* __restrict__ x, int Tp, int x_base, const __grid_constant__ PostW<C, K> pw,
                                                            float* __restrict__ y, int T, int t_begin, int t_end) {
     constexpr int TB = 512, RW = TB + K - 1, LD = RW + 2;  // outputs per block, staged rows, row stride of the staged tile
     __shared__ float sx[C][LD];
     asm volatile("griddepcontrol.wait;" ::: "memory");
     const int t0 = t_begin + blockIdx.x * TB, b = blockIdx.y, row_end = min(T + G2_PADR, x_base + Tp - G2_PADL);
+    const int lim = RAGGED ? min(t_end, pw.lens[b] * pw.lens_scale) : t_end;  // end of batch b's samples
+    if (RAGGED && t0 >= lim) {  // wholly past it: zeros, nothing computed
+        for (int t = t0 + (int)threadIdx.x; t < min(t0 + TB, t_end); t += 256) y[(size_t)b * T + t] = 0.f;
+        return;
+    }
     for (int i = threadIdx.x; i < (C / 8) * RW; i += blockDim.x) {
         const int g = i / RW, r = i - g * RW, row = t0 - K / 2 + r;  // row >= -K/2 >= -G2_PADL
         float f[8];
@@ -413,7 +438,7 @@ __global__ void __launch_bounds__(256) k_conv_post_tanh_h8(const uint4* __restri
                 for (int k = 0; k < 8; k++) acc = fmaf(sx[g * 8 + k][tl + j], pw.w[(g * 8 + k) * K + j], acc);
             }
         }
-        if (t < t_end) y[(size_t)b * T + t] = tanhf(acc);
+        if (t < t_end) y[(size_t)b * T + t] = !RAGGED || t < lim ? tanhf(acc) : 0.f;
     }
 }
 
@@ -435,7 +460,8 @@ __global__ void __launch_bounds__(256) k_g2_slide(const __grid_constant__ G2Slid
 }
 
 inline void g2_init_device() {
-    BV2_CUDA(cudaFuncSetAttribute(k_g2_conv, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    BV2_CUDA(cudaFuncSetAttribute(k_g2_conv<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    BV2_CUDA(cudaFuncSetAttribute(k_g2_conv<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
 }
 
 struct G2Epi {
@@ -446,6 +472,7 @@ struct G2Epi {
     int dil = 1;
     int t_begin = 0, t_end = -1;  // output window [t_begin, t_end) (t_end = -1: T_out); a ConvTranspose window is a multiple of its stride
     int st_override = 0;      // tests: force the super-tile size (m-tiles per CTA)
+    const int* lens = nullptr; int lens_scale = 0;  // ragged batch (G2Params::lens): frames per item (device), M-axis rows per frame
 };
 
 // Static part of the plan (fixed at weight-pack time): N tile and K chunk for a conv with `cols` output columns.
@@ -480,6 +507,8 @@ inline G2Plan g2_conv_plan(const TcConvW& w, const float* bias, const H8& x, con
     p.accumulate = e.accumulate; p.out_scale = e.out_scale; p.ups_u = w.ups_u; p.ups_cout = w.ups_cout;
     if (w.ups_u) BV2_CHECK(w.ups_cout % 8 == 0 && !e.accumulate, "g2_conv ups");
     p.T = x.T; p.K = w.K; p.dil = e.dil; p.pad = (w.K - 1) / 2 * e.dil;
+    BV2_CHECK(!e.lens || e.lens_scale >= 1, "g2_conv ragged rows per frame");
+    p.lens = e.lens; p.lens_scale = e.lens_scale;
     BV2_CHECK(p.pad <= G2_PADL && p.pad <= G2_PADR, "g2_conv padding exceeds the tensor halo");
     p.nt = w.nt; p.KC = w.KC; p.nchunks = w.nchunks;
     const int t_end = e.t_end < 0 ? y.T : e.t_end;
@@ -547,7 +576,7 @@ inline G2Plan g2_conv_plan(const TcConvW& w, const float* bias, const H8& x, con
 inline void g2_conv(const TcConvW& w, const float* bias, const H8& x, const H8& y, const G2Epi& e, cudaStream_t st, int num_sms) {
     G2Params p;
     const G2Plan pl = g2_conv_plan(w, bias, x, y, e, num_sms, p);
-    launch_pdl(k_g2_conv, pl.grid, dim3(640), pl.smem, st, p);
+    launch_pdl(p.lens ? k_g2_conv<true> : k_g2_conv<false>, pl.grid, dim3(640), pl.smem, st, p);
 }
 
 }  // namespace bv2

@@ -182,12 +182,15 @@ class Engine:
                                              float(sdp_ratio), _ptr(k[9]), self._stream(), ylen, C.byref(fmax)))
         return np.frombuffer(ylen, dtype=np.int64).copy(), int(fmax.value)
 
-    def infer_finish(self, B, T, F, noise_z, noise_scale, max_len=None, want_attn=True, out_ptr: Optional[int] = None, pcm16: bool = False):
+    def infer_finish(self, B, T, F, noise_z, noise_scale, max_len=None, want_attn=True, out_ptr: Optional[int] = None, pcm16: bool = False,
+                     ragged: bool = False):
         """`out_ptr`: raw device address that receives the waveform batch [B,1,Fg*hop] instead of a fresh tensor -- e.g. a
         slice of a peer-mapped slab (sharding.PeerWaveSlab) so the Generator epilogue stores straight into the root GPU's
         memory over NVLink; the returned `o` is then None.  `want_attn=False` skips the O(F*T) attn write (use `attn_path()`
         later if it is needed after all).  `pcm16=True`: `o` is int16, peak-normalised exactly as the reference's callers
-        convert every infer() result (gradio convert_to_16_bit_wav, webui.py:86)."""
+        convert every infer() result (gradio convert_to_16_bit_wav, webui.py:86).  `ragged=True` (FP16 Generator only, ValueError
+        otherwise): the Generator runs each utterance at its own length, so its samples are those of a run of it alone and 0 past
+        its length (bv2_infer_finish_ragged), instead of the padded batch's."""
         I, hop = self.cfg.inter_channels, self.cfg.hop
         noise_z = self._f32(noise_z)
         assert noise_z.shape[0] == B and noise_z.shape[1] == I and noise_z.shape[2] >= F
@@ -198,10 +201,14 @@ class Engine:
         y_mask = torch.empty(B, 1, F, device=dev, dtype=torch.float32)
         z, z_p, m_p, logs_p = (torch.empty(B, I, F, device=dev, dtype=torch.float32) for _ in range(4))
         self._last = (B, T, F)
-        fn = self.lib.bv2_infer_finish_pcm16 if pcm16 else self.lib.bv2_infer_finish
-        self._check(fn(self._h, _ptr(noise_z), noise_z.shape[2], float(noise_scale),
-                -1 if max_len is None else int(max_len), _ptr(o) if out_ptr is None else C.c_void_p(int(out_ptr)),
-                _ptr(attn), _ptr(y_mask), _ptr(z), _ptr(z_p), _ptr(m_p), _ptr(logs_p), self._stream()))
+        dst = _ptr(o) if out_ptr is None else C.c_void_p(int(out_ptr))
+        tail = (_ptr(attn), _ptr(y_mask), _ptr(z), _ptr(z_p), _ptr(m_p), _ptr(logs_p), self._stream())
+        head = (self._h, _ptr(noise_z), noise_z.shape[2], float(noise_scale), -1 if max_len is None else int(max_len))
+        if ragged:
+            self._check(self.lib.bv2_infer_finish_ragged(*head, None if pcm16 else dst, dst if pcm16 else None, *tail))
+        else:
+            fn = self.lib.bv2_infer_finish_pcm16 if pcm16 else self.lib.bv2_infer_finish
+            self._check(fn(*head, dst, *tail))
         return o, attn, y_mask, (z, z_p, m_p, logs_p)
 
     def infer_finish_stream(self, B, T, F, noise_z, noise_scale, max_len=None, want_attn=True, max_chunk_frames: Optional[int] = None):
@@ -278,13 +285,19 @@ class Engine:
         self._check(self.lib.bv2_flow_reverse(self._h, B, F, _ptr(k[0]), _ptr(k[1]), _ptr(k[2]), _ptr(z), self._stream()))
         return z
 
-    def generator(self, z, g, out: Optional[torch.Tensor] = None):
+    def generator(self, z, g, out: Optional[torch.Tensor] = None, lengths=None):
+        """z [B,inter,F], g [B,gin(,1)] -> [B,1,F*hop].  `lengths` [B] (frames; FP16 Generator only, ValueError otherwise): a ragged
+        batch, item b run at its own length clamped to [1, F], with zeros past it (bv2_generator_ragged)."""
         B, I, F = z.shape
         z = self._f32(z)
         g = self._f32(g.reshape(B, -1))
         if out is None:
             out = torch.empty(B, 1, F * self.cfg.hop, device=self.device)
-        self._check(self.lib.bv2_generator(self._h, B, F, _ptr(z), _ptr(g), _ptr(out), self._stream()))
+        if lengths is None:
+            self._check(self.lib.bv2_generator(self._h, B, F, _ptr(z), _ptr(g), _ptr(out), self._stream()))
+        else:
+            lens = self._i64(torch.as_tensor(lengths)).reshape(B)
+            self._check(self.lib.bv2_generator_ragged(self._h, B, F, _ptr(z), _ptr(g), _ptr(lens), _ptr(out), self._stream()))
         return out
 
     def debug_read(self, name: str, shape) -> torch.Tensor:

@@ -37,8 +37,10 @@ def pad_items(items: Sequence[Tuple[torch.Tensor, ...]], device) -> dict:
 
 @torch.no_grad()
 def infer_batch(net, items: Sequence[Tuple[torch.Tensor, ...]], sid: int, batch_size: int = 32, sdp_ratio=0.2, noise_scale=0.6,
-                noise_scale_w=0.8, length_scale=1.0) -> List[np.ndarray]:
-    """Returns one float32 waveform per item (same order), as infer.infer returns for a single slice (infer.py:315-318)."""
+                noise_scale_w=0.8, length_scale=1.0, ragged=False) -> List[np.ndarray]:
+    """Returns one float32 waveform per item (same order), as infer.infer returns for a single slice (infer.py:315-318).
+    `ragged=True` is passed to net.infer: the Generator then runs each utterance at its own length, so no utterance pays for the
+    longest one of its bucket and none sees the padding in its last frames (FP16 Generator only; see SynthesizerTrn.infer)."""
     dev = next(net.parameters()).device
     lengths = [int(it[3].shape[0]) for it in items]
     plan = deal_buckets(lengths, world_size=1, batch_size=batch_size)[0]
@@ -48,7 +50,8 @@ def infer_batch(net, items: Sequence[Tuple[torch.Tensor, ...]], sid: int, batch_
         d = pad_items([items[i] for i in bucket], dev)
         sids = torch.full((len(bucket),), int(sid), dtype=torch.int64, device=dev)
         o, _, y_mask, _ = net.infer(d["x"], d["x_lengths"], sids, d["tone"], d["language"], d["bert"], d["ja_bert"], d["en_bert"],
-                                    sdp_ratio=sdp_ratio, noise_scale=noise_scale, noise_scale_w=noise_scale_w, length_scale=length_scale)
+                                    sdp_ratio=sdp_ratio, noise_scale=noise_scale, noise_scale_w=noise_scale_w, length_scale=length_scale,
+                                    ragged=ragged)
         n = (y_mask.sum((1, 2)).long() * hop).cpu()
         wav = o[:, 0].float().cpu().numpy()
         for k, i in enumerate(bucket):

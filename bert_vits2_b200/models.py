@@ -213,12 +213,18 @@ class SynthesizerTrn(nn.Module):
     # ----------------------------------------------------------------------------------------------------
     @torch.no_grad()
     def infer(self, x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_scale=0.667, length_scale=1,
-              noise_scale_w=0.8, max_len=None, sdp_ratio=0, y=None, *, noise_w=None, noise_z=None, w_ceil_override=None, pcm16=False):
+              noise_scale_w=0.8, max_len=None, sdp_ratio=0, y=None, *, noise_w=None, noise_z=None, w_ceil_override=None, pcm16=False,
+              ragged=False):
         """reference models.py:1026-1074.  Keyword-only extras (not in the reference): explicit noise tensors
         `noise_w` [B,2,T] / `noise_z` [B,inter,>=F] replacing the two in-model RNG draws (models.py:249, 1071), and
         `w_ceil_override` [B,T] to teacher-force durations in parity harnesses, `pcm16=True` to get `o` as int16 converted like
-        the reference's callers do (gradio convert_to_16_bit_wav, webui.py:86).  `attn` comes back as a LazyAttn (see above).
+        the reference's callers do (gradio convert_to_16_bit_wav, webui.py:86).  `ragged=True` (precision fp16 / fp16g only,
+        ValueError otherwise): the Generator runs each utterance at its own length instead of the padded one, so each waveform is
+        what the utterance gives alone (its last frames do not see the padding) and 0 past its length; a different result from
+        the reference's padded batch, not a faster route to it.  `attn` comes back as a LazyAttn (see above).
         The call leases one engine of the module's pool from begin to finish (concurrency=N: up to N calls run at once)."""
+        if ragged and self.precision not in ("fp16", "fp16g"):
+            raise ValueError(f"ragged=True needs the FP16 Generator (precision fp16 or fp16g), not {self.precision}")
         dev = self._cuda_device("infer")
         if x.dim() != 2 or bert.dim() != 3 or bert.shape[-1] != x.shape[1]:
             raise ValueError("expected x [B,T] and bert features [B,1024,T]")
@@ -232,7 +238,8 @@ class SynthesizerTrn(nn.Module):
                                                length_scale, sdp_ratio, w_ceil_override)
                 if noise_z is None:  # torch.randn_like(m_p), m_p: [B, inter, F] (models.py:1071)
                     noise_z = torch.randn(B, self.inter_channels, F, device=dev, dtype=torch.float32)
-                o, _, y_mask, aux = eng.infer_finish(B, T, F, noise_z, noise_scale, max_len, want_attn=False, pcm16=pcm16)
+                extra = {"ragged": True} if ragged else {}
+                o, _, y_mask, aux = eng.infer_finish(B, T, F, noise_z, noise_scale, max_len, want_attn=False, pcm16=pcm16, **extra)
                 results += [o, y_mask, *aux]
             eng._attn_token = token = object()
         self.last_y_lengths = y_lengths

@@ -114,6 +114,14 @@ int bv2_infer_finish(bv2_engine* e, const float* noise_z, int64_t noise_ld, floa
 int bv2_infer_finish_pcm16(bv2_engine* e, const float* noise_z, int64_t noise_ld, float noise_scale, int32_t max_len,
                            int16_t* o16, float* attn, float* y_mask, float* z, float* z_p, float* m_p, float* logs_p,
                            void* stream);
+/* Ragged batch: bv2_infer_finish (o) or bv2_infer_finish_pcm16 (o16), exactly one of the two non-NULL, except that the Generator runs
+ * each utterance at its own length min(y_lengths[b], Fg) instead of the padded Fg.  Utterance b's samples [0, min(y_lengths[b], Fg)*hop)
+ * are bit-identical to a B=1 run of it at that length (bv2_generator_ragged documents the invariant); its samples past that are 0.
+ * This differs from the padded result, whose last ~14 frames of every shorter utterance see the padding's non-zero activations.
+ * Everything before the Generator, and y_mask, z, z_p, m_p, logs_p, are those of bv2_infer_finish.  Same launches and workspace
+ * (bv2_reserve covers it).  FP16 Generator only (generator_precision 2 or 3): an fp32 or TF32 Generator returns BV2_ERR_ARG. */
+int bv2_infer_finish_ragged(bv2_engine* e, const float* noise_z, int64_t noise_ld, float noise_scale, int32_t max_len, float* o,
+                            int16_t* o16, float* attn, float* y_mask, float* z, float* z_p, float* m_p, float* logs_p, void* stream);
 /* Streaming synthesis: audio leaves the Generator in chunks, before the whole utterance has gone through it.
  * bv2_infer_finish_stream does what bv2_infer_finish does up to and including the flow (same arguments and outputs), then opens a
  * stream over the caller's o [B,1,Fg*hop], which must stay allocated until the stream is closed.  Every
@@ -177,6 +185,11 @@ int bv2_flow_reverse(bv2_engine* e, int B, int F, const float* z_p, const int64_
                      float* z, void* stream);
 /* Generator: z [B,inter,F], g [B,gin] -> o [B,1,F*hop] (reference models.py:538-557)                          */
 int bv2_generator(bv2_engine* e, int B, int F, const float* z, const float* g, float* o, void* stream);
+/* Ragged Generator: item b runs at L_b = lengths[b] (int64, DEVICE [B]) clamped to [1, F] on the device.  o[b, :L_b*hop] is
+ * bit-identical to bv2_generator(B=1, F=L_b) on z[b, :, :L_b] and g[b]; o[b, L_b*hop:] is 0.  Every layer stores item b's rows below
+ * L_b times its rows per frame, then zeros in the G2_PADR rows after them (what a run at L_b has as its zero halo); work wholly past
+ * L_b is skipped.  FP16 Generator only, else BV2_ERR_ARG. */
+int bv2_generator_ragged(bv2_engine* e, int B, int F, const float* z, const float* g, const int64_t* lengths, float* o, void* stream);
 
 /* Debug tap: copy a named internal stage buffer of the LAST call (converted to [B,C,T]) to HOST memory.
  * Returns the number of floats written, or a negative status.                                               */
