@@ -25,6 +25,9 @@ BOUNDED_HARNESS_PATH = os.path.join(HERE, "libbv2_stream_bounded_harness.so")
 # ragged-batch harness (tests/cuda/ragged_harness.cu): a k_g2_conv launch whose items stop at their own lengths, on top of the kernel harness
 RAGGED_HARNESS_SOURCE = os.path.join(ROOT, "tests", "cuda", "ragged_harness.cu")
 RAGGED_HARNESS_PATH = os.path.join(HERE, "libbv2_ragged_harness.so")
+# ragged-stream harness (tests/cuda/ragged_stream_harness.cu): a k_g2_conv window of a ragged stream, on top of the bounded-stream harness
+RAGGED_STREAM_HARNESS_SOURCE = os.path.join(ROOT, "tests", "cuda", "ragged_stream_harness.cu")
+RAGGED_STREAM_HARNESS_PATH = os.path.join(HERE, "libbv2_ragged_stream_harness.so")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
 MAX_UPS, MAX_RK, MAX_DIL = 8, 4, 4
@@ -63,6 +66,8 @@ SYMBOLS = {
     "bv2_stream_advance": (C.c_int, [P, C.c_int32, C.c_void_p, C.POINTER(C.c_int64)]),
     "bv2_infer_finish_stream_bounded": (C.c_int, [P, F32P, C.c_int64, C.c_float, C.c_int32, C.c_int32, F32P, F32P, F32P, F32P, F32P, F32P, F32P,
                                                   C.c_void_p]),
+    "bv2_infer_finish_stream_ragged": (C.c_int, [P, F32P, C.c_int64, C.c_float, C.c_int32, C.c_int32, F32P, F32P, F32P, F32P, F32P, F32P, F32P,
+                                                 C.c_void_p]),
     "bv2_stream_bytes": (C.c_int64, [P, C.c_int, C.c_int32, C.c_int32]),
     "bv2_wave_to_pcm16": (C.c_int, [P, C.c_int, C.c_int64, F32P, I64P, C.c_void_p, C.c_void_p]),
     "bv2_attn_path": (C.c_int, [P, F32P, C.c_void_p]),
@@ -117,8 +122,10 @@ def build(force: bool = False, verbose: bool = False) -> str:
         return LIB_PATH
 
 
-def _harness(stream: bool, bounded: bool, ragged: bool = False):
+def _harness(stream: bool, bounded: bool, ragged: bool = False, ragged_stream: bool = False):
     """(source, library) of a test harness"""
+    if ragged_stream:
+        return RAGGED_STREAM_HARNESS_SOURCE, RAGGED_STREAM_HARNESS_PATH
     if ragged:
         return RAGGED_HARNESS_SOURCE, RAGGED_HARNESS_PATH
     if bounded:
@@ -126,21 +133,21 @@ def _harness(stream: bool, bounded: bool, ragged: bool = False):
     return (STREAM_HARNESS_SOURCE, STREAM_HARNESS_PATH) if stream else (HARNESS_SOURCE, HARNESS_PATH)
 
 
-def harness_needs_build(stream: bool = False, bounded: bool = False, ragged: bool = False) -> bool:
-    src, path = _harness(stream, bounded, ragged)
+def harness_needs_build(stream: bool = False, bounded: bool = False, ragged: bool = False, ragged_stream: bool = False) -> bool:
+    src, path = _harness(stream, bounded, ragged, ragged_stream)
     if not os.path.isfile(path):
         return True
     t = os.path.getmtime(path)
-    deps = {HARNESS_SOURCE, src} | set(HEADERS)
+    deps = {HARNESS_SOURCE, src} | set(HEADERS) | ({BOUNDED_HARNESS_SOURCE} if ragged_stream else set())
     return any(os.path.getmtime(p) > t for p in deps if os.path.isfile(p))
 
 
-def build_harness(force: bool = False, stream: bool = False, bounded: bool = False, ragged: bool = False) -> str:
+def build_harness(force: bool = False, stream: bool = False, bounded: bool = False, ragged: bool = False, ragged_stream: bool = False) -> str:
     """Compile the kernel test harness (stream=True: the streaming harness, bounded=True: the bounded-stream harness, ragged=True:
-    the ragged-batch harness) next to libbv2.so with the product flags."""
-    src, path = _harness(stream, bounded, ragged)
+    the ragged-batch harness, ragged_stream=True: the ragged-stream harness) next to libbv2.so with the product flags."""
+    src, path = _harness(stream, bounded, ragged, ragged_stream)
     with _lock:
-        if not force and not harness_needs_build(stream, bounded, ragged):
+        if not force and not harness_needs_build(stream, bounded, ragged, ragged_stream):
             return path
         tmp = path + ".tmp"
         r = subprocess.run(["nvcc"] + NVCC_FLAGS + ["-o", tmp, src], capture_output=True, text=True)

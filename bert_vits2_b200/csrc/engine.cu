@@ -152,6 +152,7 @@ struct bv2_engine : DeviceWeights {
         GenGraph g; std::vector<H8> t; std::vector<Act> a;  // tensors of the FP16 Generator (t) / of the fp32 c4 Generator (a)
         float* o = nullptr; const float* gdec = nullptr; int g_stride = 0; const int* lens = nullptr;
         int max_chunk = 0;      // > 0: bounded stream
+        bool ragged = false;    // FP16: item b runs at its own length min(lens[b], Fg) (bv2_infer_finish_stream_ragged)
         std::vector<int> rows;  // FP16: rows of storage per tensor (gen_stream_rows)
         Act z;                  // FP16: the Generator input z (fp32 c4), converted per chunk
     } gs;
@@ -405,7 +406,7 @@ struct bv2_engine : DeviceWeights {
     H8 g2_h8(int B, int C, int T, int rows = -1);
     H8 g2_input(Act z, const int* lens_or_null, cudaStream_t s);
     size_t stream_bytes(int B, int Fg, int max_chunk) const;
-    void gen_stream_open(Act z, const int* lens_or_null, const float* gdec, int g_stride, float* o, int max_chunk);
+    void gen_stream_open(Act z, const int* lens_or_null, const float* gdec, int g_stride, float* o, int max_chunk, bool ragged);
     void g2_stream_prepare(int done, int target, cudaStream_t s);
     void gen_windows(const GenGraph& g, const std::vector<GenWin>& w, std::vector<Act>& t, bool stream, const int* lens_or_null, const float* gdec,
                      int g_stride, float* o, cudaStream_t s);
@@ -1160,7 +1161,8 @@ size_t bv2_engine::stream_bytes(int B, int Fg, int max_chunk) const {
     return n;
 }
 
-void bv2_engine::gen_stream_open(Act z, const int* lens, const float* gdec, int g_stride, float* o, int max_chunk) {
+void bv2_engine::gen_stream_open(Act z, const int* lens, const float* gdec, int g_stride, float* o, int max_chunk, bool ragged) {
+    BV2_CHECK(!ragged || (use_g2 && lens), "a ragged stream needs the FP16 Generator and the lengths");
     gs.g = gen_graph(cfg, z.T);
     const size_t n = gs.g.tensor_len.size();
     gs.t.clear(); gs.a.clear(); gs.rows.clear();
@@ -1175,6 +1177,7 @@ void bv2_engine::gen_stream_open(Act z, const int* lens, const float* gdec, int 
     }
     gs.max_chunk = gen_stream_bounded(z.T, max_chunk) ? max_chunk : 0;
     gs.B = z.B; gs.Fg = z.T; gs.frontier = 0; gs.o = o; gs.gdec = gdec; gs.g_stride = g_stride; gs.lens = lens; gs.z = z;
+    gs.ragged = ragged;
     gs.open = true;
 }
 
@@ -1211,7 +1214,9 @@ void bv2_engine::g2_stream_prepare(int done, int target, cudaStream_t s) {
 // bump-allocated per stage and released after the join (the convs of one resblock chain share one temporary and two ping-pong
 // buffers).  stream = true: a chunk of a stream, on tensors that live as long as the stream and hold the rows of gen_stream_rows().
 // Every tensor is addressed by logical row through its base (0 for a whole tensor).  ragged_lens (device, frames per item; null: every
-// item has all g.tensor_len[0] frames): every layer stores item b's rows below its length only, at the layer's rows per frame.
+// item has all g.tensor_len[0] frames): every layer stores item b's rows below its length only, at the layer's rows per frame, followed
+// by its zero halo (one-shot) or, in a stream, by zeros in every later row of each window (G2_RAGGED_STREAM; conv_post and the input
+// conversion already store zeros past an item's end inside their windows and nothing outside them).
 void bv2_engine::g2_windows(const GenGraph& g, const std::vector<GenWin>& w, std::vector<H8>& t, bool stream, const float* gdec, int g_stride,
                             float* o, cudaStream_t s, const int* ragged_lens) {
     const int B = t[0].B;
@@ -1221,7 +1226,7 @@ void bv2_engine::g2_windows(const GenGraph& g, const std::vector<GenWin>& w, std
         const GenWin& wi = w[li++];
         if (wi.t_end <= wi.t_begin) return;
         e.t_begin = wi.t_begin; e.t_end = wi.t_end;
-        if (ragged_lens) { e.lens = ragged_lens; e.lens_scale = l.L_in / g.tensor_len[0]; }  // the M axis is the input's time axis
+        if (ragged_lens) { e.lens = ragged_lens; e.lens_scale = l.L_in / g.tensor_len[0]; e.ragged_stream = stream; }  // the M axis is the input's time axis
         if (l.res >= 0) e.res = &t[l.res];
         g2_conv(cw, bias, t[l.in], t[l.out], e, sj, num_sms); launches++;
     };
@@ -1515,7 +1520,8 @@ int bv2_infer_begin(bv2_engine* e, int B, int T, const int64_t* x, const int64_t
 }
 
 // open_stream: stop after the flow and open a Generator stream over o instead of running the Generator (bv2_infer_finish_stream)
-// ragged: the Generator runs each utterance at its own length (bv2_infer_finish_ragged)
+// ragged: the Generator runs each utterance at its own length (bv2_infer_finish_ragged; with open_stream, a ragged stream:
+// bv2_infer_finish_stream_ragged)
 static int infer_finish_impl(bv2_engine* e, const float* noise_z, int64_t noise_ld, float noise_scale, int32_t max_len, float* o, int16_t* o16,
                              float* attn, float* y_mask, float* z_out, float* z_p, float* m_p, float* logs_p, void* stream, bool open_stream = false,
                              int max_chunk = 0, bool ragged = false) {
@@ -1560,7 +1566,7 @@ static int infer_finish_impl(bv2_engine* e, const float* noise_z, int64_t noise_
         BV2_CUDA(cudaMemcpy2DAsync(zg.p, (size_t)Fg * 16, z.p, (size_t)F * 16, (size_t)Fg * 16, (size_t)B * I / 4, cudaMemcpyDeviceToDevice, s));
     }
     if (open_stream) {
-        e->gen_stream_open(zg, st.ylen32, st.gproj + e->goff_dec, e->gproj_n, o, max_chunk);
+        e->gen_stream_open(zg, st.ylen32, st.gproj + e->goff_dec, e->gproj_n, o, max_chunk, ragged);
         st.active = false; st.finished = true;
         return BV2_OK;
     }
@@ -1607,6 +1613,13 @@ int bv2_infer_finish_stream_bounded(bv2_engine* e, const float* noise_z, int64_t
                              std::max<int32_t>(max_chunk_frames, 0));
 }
 
+int bv2_infer_finish_stream_ragged(bv2_engine* e, const float* noise_z, int64_t noise_ld, float noise_scale, int32_t max_len, int32_t max_chunk_frames,
+                                   float* o, float* attn, float* y_mask, float* z_out, float* z_p, float* m_p, float* logs_p, void* stream) {
+    if (!o) return BV2_ERR_ARG;
+    return infer_finish_impl(e, noise_z, noise_ld, noise_scale, max_len, o, nullptr, attn, y_mask, z_out, z_p, m_p, logs_p, stream, true,
+                             std::max<int32_t>(max_chunk_frames, 0), true);
+}
+
 int bv2_infer_finish_stream(bv2_engine* e, const float* noise_z, int64_t noise_ld, float noise_scale, int32_t max_len, float* o,
                             float* attn, float* y_mask, float* z_out, float* z_p, float* m_p, float* logs_p, void* stream) {
     return bv2_infer_finish_stream_bounded(e, noise_z, noise_ld, noise_scale, max_len, 0, o, attn, y_mask, z_out, z_p, m_p, logs_p, stream);
@@ -1622,12 +1635,14 @@ int bv2_stream_advance(bv2_engine* e, int32_t frames, void* stream, int64_t* sam
     const int f = std::min<int>(frames, gs.Fg);
     const std::vector<GenWin> w = gen_stream_plan(gs.g, gs.Fg, gs.frontier, f);
     cudaStream_t s = static_cast<cudaStream_t>(stream);
+    e->stage_begin("generator", s);
     if (e->use_g2) {
         e->g2_stream_prepare(gs.frontier, f, s);
-        e->g2_windows(gs.g, w, gs.t, true, gs.gdec, gs.g_stride, gs.o, s);
+        e->g2_windows(gs.g, w, gs.t, true, gs.gdec, gs.g_stride, gs.o, s, gs.ragged ? gs.lens : nullptr);
     } else {
         e->gen_windows(gs.g, w, gs.a, true, gs.lens, gs.gdec, gs.g_stride, gs.o, s);
     }
+    e->stage_end("generator", s);
     gs.frontier = f;
     if (samples_ready) *samples_ready = (int64_t)f * e->hop;
     if (f == gs.Fg) gs.open = false;

@@ -171,17 +171,56 @@ __device__ __forceinline__ void g2_issuer_nt(const G2Issue& q, int nt, int MG) {
 template <bool RAGGED>
 __device__ __forceinline__ int g2_lim(const G2Params& p, int b) { return RAGGED ? min(p.t_end, p.lens[b] * p.lens_scale) : p.t_end; }
 
-// RAGGED = false is the kernel of a batch without lengths, compiled as if the ragged case did not exist (same registers and code).
-template <bool RAGGED>
+// Which rows of batch item b a k_g2_conv launch stores:
+//   G2_ALL            every row of the window (no lengths);
+//   G2_RAGGED         a one-shot ragged batch: the item's rows below its end lim, then G2_PADR zero rows after it (its own halo, which
+//                     may lie past the window), nothing past those;
+//   G2_RAGGED_STREAM  one window of a ragged stream: the item's rows below lim, and zeros in every row of the window at or past lim.
+//                     A halo past the window could not be kept: a bounded stream's slide keeps only the rows below need(done), and no
+//                     later window would rewrite the rest.  Stored inside the window, the zeros are final rows like any other, and a
+//                     consumer (reading at most lim * u + 25 rows) finds them whichever chunk it runs in.  Nothing is stored past the
+//                     window except the tensor's own halos, as in G2_ALL.
+enum G2Rows { G2_ALL = 0, G2_RAGGED = 1, G2_RAGGED_STREAM = 2 };
+
+// G2_RAGGED_STREAM, a CTA wholly past item b's end: zeros in its rows of the window (M-axis rows [t0, t1), this N tile's columns) and,
+// from N tile 0, in the tensor's halos that the window reaches; all 640 threads, no barrier.
+__device__ __forceinline__ void g2_zero_rows(const G2Params& p, int t0, int t1, int n0, int b) {
+    asm volatile("griddepcontrol.wait;" ::: "memory");  // the rows may alias rows an upstream kernel still reads or slides
+    const uint4 z4 = make_uint4(0u, 0u, 0u, 0u);
+    const int u = p.ups_u, rows = t1 - t0;
+    for (int i = threadIdx.x; i < rows * (p.nt / 8); i += blockDim.x) {
+        const int h = i / rows, t = t0 + (i - h * rows), n = n0 + 8 * h;  // 8 consecutive output columns from n, M-axis row t
+        size_t yo;
+        if (u) { const int r = n / p.ups_cout, co = n - r * p.ups_cout; yo = ((size_t)b * p.y_cg + co / 8) * p.y_Tp + (size_t)t * u + r; }
+        else yo = ((size_t)b * p.y_cg + n / 8) * p.y_Tp + t;
+        p.y[yo] = z4;
+    }
+    if (blockIdx.y != 0) return;
+    uint4* yb = p.y + (size_t)b * p.y_cg * p.y_Tp;
+    if (blockIdx.x == 0 && p.t_begin == 0)
+        for (int i = threadIdx.x; i < p.y_cg * G2_PADL; i += blockDim.x) yb[(size_t)(i / G2_PADL) * p.y_Tp + (i % G2_PADL) - G2_PADL] = z4;
+    if (blockIdx.x == gridDim.x - 1 && p.t_end == p.T) {
+        const int hrow = p.T * (u ? u : 1);
+        for (int i = threadIdx.x; i < p.y_cg * G2_PADR; i += blockDim.x) yb[(size_t)(i / G2_PADR) * p.y_Tp + hrow + (i % G2_PADR)] = z4;
+    }
+}
+
+// ROWS = G2_ALL is the kernel of a batch without lengths, compiled as if the ragged cases did not exist (same registers and code).
+template <int ROWS>
 __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
     using namespace tc;
+    constexpr bool RAGGED = ROWS != G2_ALL, STREAM = ROWS == G2_RAGGED_STREAM;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = smem_raw + acc_img_bytes(p.acc_cols);  // behind the accumulator image
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;  // shfl: warp-uniform for the compiler
     const int NAS = p.nas, NWS = p.nws, NG = p.NG, MG = p.MG, NCH = p.nchunks, nt = p.nt, R = p.R;
     const int t0 = p.t_begin + blockIdx.x * NG * MG * 128, ntile = blockIdx.y, n0 = ntile * nt, b = blockIdx.z;
-    // a CTA wholly past the end of batch b's rows has nothing to store and no halo to clear (CTA-uniform exit before any barrier)
-    if (RAGGED && t0 >= g2_lim<RAGGED>(p, b)) return;
+    // a CTA wholly past the end of batch b's rows computes nothing (CTA-uniform exit before any barrier).  One-shot: it has nothing to
+    // store and no halo to clear.  Stream: it stores zeros in its rows of the window.
+    if (RAGGED && t0 >= g2_lim<RAGGED>(p, b)) {
+        if (STREAM) g2_zero_rows(p, t0, min(t0 + NG * MG * 128, p.t_end), n0, b);
+        return;
+    }
     uint8_t* sA = smem;
     uint8_t* sW = smem + (size_t)NAS * p.a_stage_bytes;
     const int nwst = p.resident ? NCH * p.K : NWS;  // weight stages held in shared memory
@@ -287,16 +326,18 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
         // ===== zero halo of the OUTPUT tensor (= the conv padding of its consumers), written by its producer: the CTA of the first super-tile
         // clears rows [-G2_PADL, 0) if the window starts at t = 0, the CTA of the last one rows [T_out, T_out + G2_PADR) if the window ends at
         // T_out, for every channel group of batch b (N tile 0 only).  A window inside the tensor leaves the halo rows alone: in a streamed run
-        // they are final rows of earlier windows.  In a ragged batch the trailing halo of item b follows its own rows: the CTA holding row
-        // lim - 1 clears output rows [lim * u, lim * u + G2_PADR) (with lim == T, the tensor's halo).
-        const int lim = g2_lim<RAGGED>(p, b);
+        // they are final rows of earlier windows.  In a one-shot ragged batch the trailing halo of item b follows its own rows: the CTA
+        // holding row lim - 1 clears output rows [lim * u, lim * u + G2_PADR) (with lim == T, the tensor's halo).  A ragged stream clears
+        // the tensor's halos as G2_ALL does; the epilogue stores the zeros after item b's end inside the window.
+        constexpr bool ONE_SHOT = RAGGED && !STREAM;
+        const int lim = g2_lim<ONE_SHOT>(p, b);
         const bool lo = blockIdx.x == 0 && p.t_begin == 0;
-        const bool hi = RAGGED ? (lim - 1 - p.t_begin) / (NG * MG * 128) == (int)blockIdx.x && (lim < p.t_end || p.t_end == p.T)
-                               : blockIdx.x == gridDim.x - 1 && p.t_end == p.T;
+        const bool hi = ONE_SHOT ? (lim - 1 - p.t_begin) / (NG * MG * 128) == (int)blockIdx.x && (lim < p.t_end || p.t_end == p.T)
+                                 : blockIdx.x == gridDim.x - 1 && p.t_end == p.T;
         if (ntile == 0 && (lo || hi)) {
             asm volatile("griddepcontrol.wait;" ::: "memory");  // the rows may alias a tensor an upstream kernel is still reading
             uint4* yb = p.y + (size_t)b * p.y_cg * p.y_Tp;
-            const int hrow = (RAGGED ? lim : p.T) * (p.ups_u ? p.ups_u : 1);
+            const int hrow = (ONE_SHOT ? lim : p.T) * (p.ups_u ? p.ups_u : 1);
             const uint4 z4 = make_uint4(0u, 0u, 0u, 0u);
             if (lo)
                 for (int i = lane; i < p.y_cg * G2_PADL; i += 32) yb[(size_t)(i / G2_PADL) * p.y_Tp + (i % G2_PADL) - G2_PADL] = z4;
@@ -337,7 +378,14 @@ __global__ void __launch_bounds__(640, 1) k_g2_conv(G2Params p) {
                         if (p.accumulate && ok) a4[h] = p.y[yo[h]];
                     }
                 }
-                if (!ok) continue;
+                if (!ok) {
+                    if (STREAM && t < p.t_end) {  // a ragged stream's row at or past item b's end, inside the window: zero
+#pragma unroll
+                        for (int h = 0; h < 4; h++)
+                            if (8 * h < cw) p.y[yo[h]] = make_uint4(0u, 0u, 0u, 0u);
+                    }
+                    continue;
+                }
 #pragma unroll
                 for (int h = 0; h < 4; h++) {
                     if (8 * h < cw) {
@@ -460,8 +508,9 @@ __global__ void __launch_bounds__(256) k_g2_slide(const __grid_constant__ G2Slid
 }
 
 inline void g2_init_device() {
-    BV2_CUDA(cudaFuncSetAttribute(k_g2_conv<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    BV2_CUDA(cudaFuncSetAttribute(k_g2_conv<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    BV2_CUDA(cudaFuncSetAttribute(k_g2_conv<G2_ALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    BV2_CUDA(cudaFuncSetAttribute(k_g2_conv<G2_RAGGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    BV2_CUDA(cudaFuncSetAttribute(k_g2_conv<G2_RAGGED_STREAM>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
 }
 
 struct G2Epi {
@@ -473,6 +522,7 @@ struct G2Epi {
     int t_begin = 0, t_end = -1;  // output window [t_begin, t_end) (t_end = -1: T_out); a ConvTranspose window is a multiple of its stride
     int st_override = 0;      // tests: force the super-tile size (m-tiles per CTA)
     const int* lens = nullptr; int lens_scale = 0;  // ragged batch (G2Params::lens): frames per item (device), M-axis rows per frame
+    int ragged_stream = 0;    // with lens: the launch is one window of a ragged stream (G2_RAGGED_STREAM)
 };
 
 // Static part of the plan (fixed at weight-pack time): N tile and K chunk for a conv with `cols` output columns.
@@ -576,7 +626,8 @@ inline G2Plan g2_conv_plan(const TcConvW& w, const float* bias, const H8& x, con
 inline void g2_conv(const TcConvW& w, const float* bias, const H8& x, const H8& y, const G2Epi& e, cudaStream_t st, int num_sms) {
     G2Params p;
     const G2Plan pl = g2_conv_plan(w, bias, x, y, e, num_sms, p);
-    launch_pdl(p.lens ? k_g2_conv<true> : k_g2_conv<false>, pl.grid, dim3(640), pl.smem, st, p);
+    BV2_CHECK(!e.ragged_stream || p.lens, "g2_conv: a ragged stream window without lengths");
+    launch_pdl(!p.lens ? k_g2_conv<G2_ALL> : e.ragged_stream ? k_g2_conv<G2_RAGGED_STREAM> : k_g2_conv<G2_RAGGED>, pl.grid, dim3(640), pl.smem, st, p);
 }
 
 }  // namespace bv2

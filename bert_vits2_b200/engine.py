@@ -211,12 +211,15 @@ class Engine:
             self._check(fn(*head, dst, *tail))
         return o, attn, y_mask, (z, z_p, m_p, logs_p)
 
-    def infer_finish_stream(self, B, T, F, noise_z, noise_scale, max_len=None, want_attn=True, max_chunk_frames: Optional[int] = None):
+    def infer_finish_stream(self, B, T, F, noise_z, noise_scale, max_len=None, want_attn=True, max_chunk_frames: Optional[int] = None,
+                            ragged: bool = False):
         """infer_finish up to and including the flow, then open a Generator stream over the returned `o` [B,1,Fg*hop]; its samples become
         final as stream_advance() is called.  Returns (o, attn, y_mask, (z, z_p, m_p, logs_p)) like infer_finish.  Every precision;
         no pcm16 (its peak normalisation needs the whole utterance).  `max_chunk_frames`: a cap on how far one stream_advance may
         move the frontier; below Fg it bounds the stream's Generator memory (stream_bytes) and needs the FP16 Generator (ValueError
-        otherwise)."""
+        otherwise).  `ragged=True` (FP16 Generator only, ValueError otherwise): the Generator runs each utterance at its own length
+        L_b = min(y_lengths[b], Fg), so once the frontier reaches L_b its samples are those of infer_finish(..., ragged=True) and 0
+        past L_b*hop (bv2_infer_finish_stream_ragged); same chunks, launches and workspace as the padded stream."""
         I, hop = self.cfg.inter_channels, self.cfg.hop
         noise_z = self._f32(noise_z)
         assert noise_z.shape[0] == B and noise_z.shape[1] == I and noise_z.shape[2] >= F
@@ -227,9 +230,9 @@ class Engine:
         y_mask = torch.empty(B, 1, F, device=dev, dtype=torch.float32)
         z, z_p, m_p, logs_p = (torch.empty(B, I, F, device=dev, dtype=torch.float32) for _ in range(4))
         self._last = (B, T, F)
-        self._check(self.lib.bv2_infer_finish_stream_bounded(self._h, _ptr(noise_z), noise_z.shape[2], float(noise_scale),
-                                                             -1 if max_len is None else int(max_len), _cap(max_chunk_frames), _ptr(o), _ptr(attn),
-                                                             _ptr(y_mask), _ptr(z), _ptr(z_p), _ptr(m_p), _ptr(logs_p), self._stream()))
+        fn = self.lib.bv2_infer_finish_stream_ragged if ragged else self.lib.bv2_infer_finish_stream_bounded
+        self._check(fn(self._h, _ptr(noise_z), noise_z.shape[2], float(noise_scale), -1 if max_len is None else int(max_len),
+                       _cap(max_chunk_frames), _ptr(o), _ptr(attn), _ptr(y_mask), _ptr(z), _ptr(z_p), _ptr(m_p), _ptr(logs_p), self._stream()))
         self._stream_o = o  # the stream writes into o until it closes
         return o, attn, y_mask, (z, z_p, m_p, logs_p)
 

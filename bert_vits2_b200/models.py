@@ -248,7 +248,7 @@ class SynthesizerTrn(nn.Module):
     @torch.no_grad()
     def infer_stream(self, x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_scale=0.667, length_scale=1,
                      noise_scale_w=0.8, max_len=None, sdp_ratio=0, y=None, *, noise_w=None, noise_z=None, w_ceil_override=None,
-                     first_chunk_frames=32, max_chunk_frames=None):
+                     first_chunk_frames=32, max_chunk_frames=None, ragged=False):
         """Streaming infer(): a generator of waveform chunks o[:, :, a:b] (device tensors, views of one [B,1,Fg*hop] buffer) whose
         concatenation is bit-identical to infer(...)[0] with the same noise.  Encoder, durations and flow run whole first (the flow's
         attention spans the utterance); the Generator then runs as a wavefront, so the first chunk costs about first_chunk_frames
@@ -259,7 +259,12 @@ class SynthesizerTrn(nn.Module):
         `max_chunk_frames`: chunks double only up to this many frames, and the stream's Generator memory is then set by it, not by
         the utterance's length (bounded stream: Engine.stream_bytes).  It needs the FP16 Generator (precision fp16 or fp16g) when it
         is below the utterance's frame count; ValueError otherwise, and for max_chunk_frames < first_chunk_frames.  None: chunks
-        double without limit and every Generator activation stays resident until the stream ends."""
+        double without limit and every Generator activation stays resident until the stream ends.
+        `ragged=True` (precision fp16 / fp16g only, ValueError otherwise): the Generator runs each utterance at its own length, as
+        infer(..., ragged=True) does, with the same chunks.  Utterance b's samples are final and complete once a chunk ends at or past
+        last_y_lengths[b] * hop (max_len applied), and the concatenation is bit-identical to infer(..., ragged=True)[0]: 0 past its end."""
+        if ragged and self.precision not in ("fp16", "fp16g"):
+            raise ValueError(f"ragged=True needs the FP16 Generator (precision fp16 or fp16g), not {self.precision}")
         dev = self._cuda_device("infer_stream")
         if x.dim() != 2 or bert.dim() != 3 or bert.shape[-1] != x.shape[1]:
             raise ValueError("expected x [B,T] and bert features [B,1024,T]")
@@ -279,8 +284,10 @@ class SynthesizerTrn(nn.Module):
                                                length_scale, sdp_ratio, w_ceil_override)
                 if noise_z is None:
                     noise_z = torch.randn(B, self.inter_channels, F, device=dev, dtype=torch.float32)
-                cap = {} if max_chunk_frames is None else {"max_chunk_frames": max_chunk_frames}
-                o, _, _, _ = eng.infer_finish_stream(B, T, F, noise_z, noise_scale, max_len, want_attn=False, **cap)
+                extra = {} if max_chunk_frames is None else {"max_chunk_frames": max_chunk_frames}
+                if ragged:
+                    extra["ragged"] = True
+                o, _, _, _ = eng.infer_finish_stream(B, T, F, noise_z, noise_scale, max_len, want_attn=False, **extra)
                 results.append(o)
             eng._attn_token = object()  # a LazyAttn of an earlier infer() must not materialise this utterance's path
             self.last_y_lengths = y_lengths

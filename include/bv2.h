@@ -148,6 +148,15 @@ int bv2_stream_advance(bv2_engine* e, int32_t frames, void* stream, int64_t* sam
 int bv2_infer_finish_stream_bounded(bv2_engine* e, const float* noise_z, int64_t noise_ld, float noise_scale, int32_t max_len,
                                     int32_t max_chunk_frames, float* o, float* attn, float* y_mask, float* z, float* z_p, float* m_p,
                                     float* logs_p, void* stream);
+/* Ragged stream: bv2_infer_finish_stream_bounded (same arguments; max_chunk_frames <= 0: unbounded) whose Generator runs each utterance
+ * at its own length L_b = min(y_lengths[b], Fg), as bv2_infer_finish_ragged does.  Once the frontier reaches L_b frames, o[b, :L_b*hop]
+ * is final and bit-identical to bv2_infer_finish_ragged's, and o[b, L_b*hop:] is 0 as far as the frontier has gone.  Every window
+ * stores the rows of an item at or past its end as zeros, so a bounded stream's slides carry them like any other final rows.  The
+ * windows, slides, launches and workspace are those of the padded stream with the same chunks (bv2_stream_bytes and
+ * bv2_reserve_stream cover it).  FP16 Generator only (generator_precision 2 or 3): an fp32 or TF32 Generator returns BV2_ERR_ARG. */
+int bv2_infer_finish_stream_ragged(bv2_engine* e, const float* noise_z, int64_t noise_ld, float noise_scale, int32_t max_len,
+                                   int32_t max_chunk_frames, float* o, float* attn, float* y_mask, float* z, float* z_p, float* m_p,
+                                   float* logs_p, void* stream);
 /* Workspace bytes of the Generator tensors of a stream over Fg frames of a batch of B with chunks of at most max_chunk_frames: for a
  * cap in [1, Fg) the bounded storage, which does not depend on Fg; else what an unbounded stream allocates.  Negative (a BV2_ERR_*
  * code) for bad arguments, an engine that is not finalized, or a cap in [1, Fg) on an fp32 / TF32 Generator. */
@@ -197,7 +206,8 @@ int64_t bv2_debug_read(bv2_engine* e, const char* name, float* host_out, int64_t
 
 /* Stage timing (CUDA events recorded on the caller's stream around "encoder_duration", "flow", "generator"):
  * enable with bv2_set_profiling(e, 1); bv2_stage_ms blocks on the stage's end event and returns the duration of
- * the stage in the LAST call, or a negative value if it was not recorded. */
+ * the stage in the LAST call, or a negative value if it was not recorded.  Each bv2_stream_advance records "generator" around the
+ * Generator work of its own chunk. */
 int bv2_set_profiling(bv2_engine* e, int enable);
 float bv2_stage_ms(bv2_engine* e, const char* stage);
 
