@@ -132,6 +132,7 @@ struct bv2_engine : DeviceWeights {
         bool active = false, finished = false; int B = 0, T = 0, F = 0;
         float* stats = nullptr; int* cum = nullptr; long long* ylen = nullptr; int* ylen32 = nullptr; int* lens = nullptr;
         float* gproj = nullptr; float* w_ceil = nullptr;
+        float* noise_scale = nullptr;  // [B] per-item noise scale of bv2_infer_begin_items (persist arena), nullptr after bv2_infer_begin
     } st;
     // Open Generator stream (bv2_infer_finish_stream .. the bv2_stream_advance that reaches Fg).  Every tensor of the Generator stays
     // in the workspace for the stream's lifetime, because later windows read the rows behind each layer's done pointer: the input z
@@ -396,8 +397,8 @@ struct bv2_engine : DeviceWeights {
     void run_dds(const DdsW& D, Act x, const int* lens, cudaStream_t s);
     void run_text_encoder(int B, int T, const int64_t* x, const int64_t* tone, const int64_t* lang, const float* bert,
                           const float* ja, const float* en, const int* lens, const float* gproj, Act& h, Act& stats, cudaStream_t s);
-    void run_durations(Act h, const int* lens, const float* gproj, const float* noise_w, float nsw, float* z, Act& dp_out, int* zch,
-                       cudaStream_t s);
+    void run_durations(Act h, const int* lens, const float* gproj, const float* noise_w, float nsw, const float* nsw_b, float* z,
+                       Act& dp_out, int* zch, cudaStream_t s);
     void run_dp(Act h, const int* lens, const float* gproj, Act& dp_out, Act xg, Act d1, Act d2, cudaStream_t s);
     void run_flow(Act z, const int* lens, const float* gproj, cudaStream_t s);
     // ragged: batch item b runs at its own length lens[b] (clamped to z.T) instead of z.T: FP16 Generator only, else BV2_ERR_ARG
@@ -484,9 +485,13 @@ __global__ void k_lengths_clamp(const long long* __restrict__ a, int* __restrict
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) b[i] = (int)max(1ll, min((long long)hi, a[i]));
 }
-__global__ void k_scale_copy(const float* __restrict__ a, float* __restrict__ b, float s, size_t n) {
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) b[i] = a[i] * s;
+// b = a * s over blockIdx.y = item rows of per_item elements; s_item ([items], bv2_infer_begin_items): item y's own s
+__global__ void k_scale_copy(const float* __restrict__ a, float* __restrict__ b, float s, const float* __restrict__ s_item, int per_item) {
+    int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= per_item) return;
+    size_t i = (size_t)blockIdx.y * per_item + j;
+    if (s_item) s = s_item[blockIdx.y];
+    b[i] = a[i] * s;
 }
 
 int* bv2_engine::lens_to_device(const int64_t* xl, int B, Arena& ar, cudaStream_t s) {
@@ -889,8 +894,8 @@ void bv2_engine::run_text_encoder(int B, int T, const int64_t* x, const int64_t*
 }
 
 // StochasticDurationPredictor(reverse) + DurationPredictor (reference models.py:197-204,245-256, 285-299)
-void bv2_engine::run_durations(Act h, const int* lens, const float* gproj, const float* noise_w, float nsw, float* z, Act& dp_out,
-                               int* zch_out, cudaStream_t s) {
+void bv2_engine::run_durations(Act h, const int* lens, const float* gproj, const float* noise_w, float nsw, const float* nsw_b, float* z,
+                               Act& dp_out, int* zch_out, cudaStream_t s) {
     const int B = h.B, T = h.T, Cf = cfg.sdp_filter;
     // ---- DP on a side stream (buffers allocated before the SDP's stack-disciplined temporaries)
     ensure_side_streams();
@@ -911,8 +916,7 @@ void bv2_engine::run_durations(Act h, const int* lens, const float* gproj, const
     if (!tok_conv(sdp_proj, c, cond, s, a1)) conv(sdp_proj, c, cond, s, a1, 0, 0, true);
     debug("sdp_cond", cond);
     {
-        size_t n = (size_t)B * 2 * T;
-        k_scale_copy<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(noise_w, z, nsw, n);
+        k_scale_copy<<<dim3(cdiv(2 * T, 256), B), 256, 0, s>>>(noise_w, z, nsw, nsw_b, 2 * T);
         BV2_CUDA(cudaGetLastError()); launches++;
     }
     Act hh = ws.act(B, Cf, T), pp = ws.act(B, 32, T);
@@ -1462,14 +1466,20 @@ int bv2_load_packed(bv2_engine* e, const char* path) {
     BV2_API_END(e)
 }
 
-int bv2_infer_begin(bv2_engine* e, int B, int T, const int64_t* x, const int64_t* x_lengths, const int64_t* sid,
-                    const int64_t* tone, const int64_t* language, const float* bert, const float* ja_bert,
-                    const float* en_bert, const float* noise_w, float noise_scale_w, float length_scale, float sdp_ratio,
-                    const float* w_ceil_override, void* stream, int64_t* y_lengths_host, int32_t* f_max) {
+// items: the settings are per-item device arrays [B] (bv2_infer_begin_items) instead of the scalars, which are then ignored
+struct ItemSettings { const float *noise_scale_w, *length_scale, *sdp_ratio, *noise_scale; };
+
+static int infer_begin_impl(bv2_engine* e, int B, int T, const int64_t* x, const int64_t* x_lengths, const int64_t* sid,
+                            const int64_t* tone, const int64_t* language, const float* bert, const float* ja_bert,
+                            const float* en_bert, const float* noise_w, float noise_scale_w, float length_scale, float sdp_ratio,
+                            const ItemSettings* items, const float* w_ceil_override, void* stream, int64_t* y_lengths_host,
+                            int32_t* f_max) {
     BV2_API_BEGIN(e)
     BV2_CHECK(e->finalized, "not finalized");
     BV2_CHECK(B >= 1 && B <= 4096 && T >= 1 && x && x_lengths && sid && tone && language && bert && ja_bert && en_bert && noise_w &&
                   y_lengths_host && f_max, "infer_begin args");
+    if (items && !(items->noise_scale_w && items->length_scale && items->sdp_ratio && items->noise_scale))
+        throw Error(BV2_ERR_ARG, "infer_begin_items: every setting array must be given");
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const bv2_config& c = e->cfg;
     const int H = c.hidden_channels, I = c.inter_channels;
@@ -1483,6 +1493,11 @@ int bv2_infer_begin(bv2_engine* e, int B, int T, const int64_t* x, const int64_t
     e->stage_begin("encoder_duration", s);
     st.ylen = reinterpret_cast<long long*>(e->persist.alloc(2 * (size_t)B + 4));  // [B] y_lengths, then the input-validation mask
     int* err_dev = reinterpret_cast<int*>(st.ylen + B);
+    st.noise_scale = nullptr;
+    if (items) {  // finish reads it; a copy, not a kernel, so the launches are those of bv2_infer_begin
+        st.noise_scale = e->persist.alloc(B);
+        BV2_CUDA(cudaMemcpyAsync(st.noise_scale, items->noise_scale, (size_t)B * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    }
     e->launch_validate(B, T, x, tone, language, sid, x_lengths, err_dev, s);
     st.lens = e->lens_to_device(x_lengths, B, e->persist, s);
     float* g = e->persist.alloc((size_t)B * c.gin_channels);
@@ -1498,12 +1513,12 @@ int bv2_infer_begin(bv2_engine* e, int B, int T, const int64_t* x, const int64_t
     float* z = e->ws.alloc((size_t)B * 2 * T);
     Act dp = e->ws.act(B, 4, T);
     int zch = 0;
-    e->run_durations(h, st.lens, st.gproj, noise_w, noise_scale_w, z, dp, &zch, s);
+    e->run_durations(h, st.lens, st.gproj, noise_w, noise_scale_w, items ? items->noise_scale_w : nullptr, z, dp, &zch, s);
     float* lsdp = e->ws.alloc((size_t)B * T); float* ldp = e->ws.alloc((size_t)B * T);
     st.w_ceil = e->persist.alloc((size_t)B * T);
     st.cum = reinterpret_cast<int*>(e->persist.alloc((size_t)B * T));
-    k_durations<<<B, 1024, 0, s>>>(z, zch, e->ea_m[0], e->ea_logs[0], dp.p, sdp_ratio, length_scale, st.lens, T, lsdp, ldp, st.w_ceil,
-                                   st.cum, st.ylen, w_ceil_override);
+    k_durations<<<B, 1024, 0, s>>>(z, zch, e->ea_m[0], e->ea_logs[0], dp.p, sdp_ratio, length_scale, items ? items->sdp_ratio : nullptr,
+                                   items ? items->length_scale : nullptr, st.lens, T, lsdp, ldp, st.w_ceil, st.cum, st.ylen, w_ceil_override);
     BV2_CUDA(cudaGetLastError()); e->launches++;
     e->debug_plain("logw_sdp", lsdp, B, 1, T); e->debug_plain("logw_dp", ldp, B, 1, T); e->debug_plain("w_ceil", st.w_ceil, B, 1, T);
     e->stage_end("encoder_duration", s);
@@ -1517,6 +1532,24 @@ int bv2_infer_begin(bv2_engine* e, int B, int T, const int64_t* x, const int64_t
     st.ylen32 = e->lens_to_device(reinterpret_cast<const int64_t*>(st.ylen), B, e->persist, s);
     st.active = true;
     BV2_API_END(e)
+}
+
+int bv2_infer_begin(bv2_engine* e, int B, int T, const int64_t* x, const int64_t* x_lengths, const int64_t* sid,
+                    const int64_t* tone, const int64_t* language, const float* bert, const float* ja_bert,
+                    const float* en_bert, const float* noise_w, float noise_scale_w, float length_scale, float sdp_ratio,
+                    const float* w_ceil_override, void* stream, int64_t* y_lengths_host, int32_t* f_max) {
+    return infer_begin_impl(e, B, T, x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_w, noise_scale_w, length_scale,
+                            sdp_ratio, nullptr, w_ceil_override, stream, y_lengths_host, f_max);
+}
+
+int bv2_infer_begin_items(bv2_engine* e, int B, int T, const int64_t* x, const int64_t* x_lengths, const int64_t* sid,
+                          const int64_t* tone, const int64_t* language, const float* bert, const float* ja_bert,
+                          const float* en_bert, const float* noise_w, const float* noise_scale_w, const float* length_scale,
+                          const float* sdp_ratio, const float* noise_scale, const float* w_ceil_override, void* stream,
+                          int64_t* y_lengths_host, int32_t* f_max) {
+    const ItemSettings items{noise_scale_w, length_scale, sdp_ratio, noise_scale};
+    return infer_begin_impl(e, B, T, x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_w, 1.f, 1.f, 0.f, &items,
+                            w_ceil_override, stream, y_lengths_host, f_max);
 }
 
 // open_stream: stop after the flow and open a Generator stream over o instead of running the Generator (bv2_infer_finish_stream)
@@ -1543,7 +1576,7 @@ static int infer_finish_impl(bv2_engine* e, const float* noise_z, int64_t noise_
     {
         dim3 grid(cdiv(F, 128), I / 4, B);
         k_expand_prior<<<grid, 128, 0, s>>>(st.stats, st.cum, st.ylen, st.lens, noise_z, (long long)I * noise_ld, (int)noise_ld, noise_scale,
-                                            I, T, F, m_tmp, l_tmp, zp_tmp, z.p, y_mask);
+                                            st.noise_scale, I, T, F, m_tmp, l_tmp, zp_tmp, z.p, y_mask);
         BV2_CUDA(cudaGetLastError()); e->launches++;
     }
     if (attn) {
@@ -1761,11 +1794,12 @@ int bv2_duration(bv2_engine* e, int B, int T, const float* x, const int64_t* x_l
     float* z = e->ws.alloc((size_t)B * 2 * T);
     Act dp = e->ws.act(B, 4, T);
     int zch = 0;
-    e->run_durations(h, lens, gp, noise_w, noise_scale_w, z, dp, &zch, s);
+    e->run_durations(h, lens, gp, noise_w, noise_scale_w, nullptr, z, dp, &zch, s);
     float* wc = e->ws.alloc((size_t)B * T);
     int* cum = reinterpret_cast<int*>(e->ws.alloc((size_t)B * T));
     long long* yl = reinterpret_cast<long long*>(e->ws.alloc(2 * (size_t)B + 2));
-    k_durations<<<B, 1024, 0, s>>>(z, zch, e->ea_m[0], e->ea_logs[0], dp.p, 0.5f, 1.f, lens, T, logw_sdp, logw_dp, wc, cum, yl, nullptr);
+    k_durations<<<B, 1024, 0, s>>>(z, zch, e->ea_m[0], e->ea_logs[0], dp.p, 0.5f, 1.f, nullptr, nullptr, lens, T, logw_sdp, logw_dp, wc, cum, yl,
+                                   nullptr);
     BV2_CUDA(cudaGetLastError()); e->launches++;
     BV2_API_END(e)
 }

@@ -759,9 +759,11 @@ __global__ void k_spline_inverse(const float* __restrict__ h, int HC, float* __r
 // ------------------------------------------------------------------------------------------------
 // Durations (reference models.py:1052-1057 + ElementwiseAffine reverse modules.py:397-399).  One block per b.
 // z: SDP latent [B][2][T] (channel `zch` is logw after the final Flip bookkeeping); dp: c4 [B][4/4][T][4] ch 0.
+// sdp_ratio_b / length_scale_b (optional, [B]): item b's own setting instead of the scalar (bv2_infer_begin_items).
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(1024) k_durations(const float* __restrict__ z, int zch, float ea_m, float ea_logs,
                                                    const float* __restrict__ dp, float sdp_ratio, float length_scale,
+                                                   const float* __restrict__ sdp_ratio_b, const float* __restrict__ length_scale_b,
                                                    const int* __restrict__ lens, int T, float* __restrict__ logw_sdp,
                                                    float* __restrict__ logw_dp, float* __restrict__ w_ceil,
                                                    int* __restrict__ cum, long long* __restrict__ y_len,
@@ -770,6 +772,8 @@ __global__ void __launch_bounds__(1024) k_durations(const float* __restrict__ z,
     __shared__ int s_carry;
     const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int len = lens[b];
+    if (sdp_ratio_b) sdp_ratio = sdp_ratio_b[b];
+    if (length_scale_b) length_scale = length_scale_b[b];
     if (tid == 0) s_carry = 0;
     __syncthreads();
     for (int t0 = 0; t0 < T; t0 += 1024) {
@@ -823,15 +827,17 @@ __global__ void __launch_bounds__(1024) k_durations(const float* __restrict__ z,
 // Length regulation + prior sampling (reference models.py:1058-1071, commons.py:126-140): a gather by
 // binary search on the duration cumsum instead of the reference's dense one-hot matmul.
 // stats: c4 [B][2I/4][T][4] (m = channels [0,I), logs = [I,2I)).  One thread per (b, f, cg).
+// noise_scale_b (optional, [B]): item b samples with noise_scale * noise_scale_b[b], rounded once (bv2_infer_begin_items).
 // ------------------------------------------------------------------------------------------------
 __global__ void k_expand_prior(const float* __restrict__ stats, const int* __restrict__ cum, const long long* __restrict__ y_len,
                                const int* __restrict__ lens, const float* __restrict__ noise, long long noise_bstride,
-                               int noise_ld, float noise_scale, int I, int T, int F, float* __restrict__ m_out,
-                               float* __restrict__ logs_out, float* __restrict__ zp_out, float* __restrict__ zp_c4,
-                               float* __restrict__ y_mask) {
+                               int noise_ld, float noise_scale, const float* __restrict__ noise_scale_b, int I, int T, int F,
+                               float* __restrict__ m_out, float* __restrict__ logs_out, float* __restrict__ zp_out,
+                               float* __restrict__ zp_c4, float* __restrict__ y_mask) {
     int f = blockIdx.x * blockDim.x + threadIdx.x;
     int cg = blockIdx.y, b = blockIdx.z;
     if (f >= F) return;
+    if (noise_scale_b) noise_scale = __fmul_rn(noise_scale, noise_scale_b[b]);
     const int yl = (int)y_len[b];
     const int* cb = cum + (size_t)b * T;
     float4 m = make_float4(0.f, 0.f, 0.f, 0.f), lg = m;

@@ -169,7 +169,11 @@ class Engine:
 
     # ---- whole path ---------------------------------------------------------------------------------
     def infer_begin(self, x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_w, noise_scale_w, length_scale,
-                    sdp_ratio, w_ceil_override=None):
+                    sdp_ratio, w_ceil_override=None, *, item_noise_scale=None):
+        """noise_scale_w, length_scale and sdp_ratio: a float, or a [B] tensor of per-utterance values.  `item_noise_scale` [B]: each
+        utterance's prior-noise scale, multiplied (rounded once) into the noise_scale every infer_finish* takes, so pass 1.0 there.
+        With any tensor this is bv2_infer_begin_items (floats broadcast to [B], item_noise_scale 1.0 when None), and utterance b comes
+        out bit-identical to a call with its own values as floats; with floats alone it is bv2_infer_begin."""
         B, T = x.shape
         self._keep = [self._i64(x), self._i64(x_lengths), self._i64(sid), self._i64(tone), self._i64(language),
                       self._f32(bert), self._f32(ja_bert), self._f32(en_bert), self._f32(noise_w),
@@ -177,10 +181,24 @@ class Engine:
         k = self._keep
         ylen = (C.c_int64 * B)()
         fmax = C.c_int32(0)
-        self._check(self.lib.bv2_infer_begin(self._h, B, T, _ptr(k[0]), _ptr(k[1]), _ptr(k[2]), _ptr(k[3]), _ptr(k[4]), _ptr(k[5]),
-                                             _ptr(k[6]), _ptr(k[7]), _ptr(k[8]), float(noise_scale_w), float(length_scale),
-                                             float(sdp_ratio), _ptr(k[9]), self._stream(), ylen, C.byref(fmax)))
+        head = (self._h, B, T, *(_ptr(t) for t in k[:9]))
+        tail = (_ptr(k[9]), self._stream(), ylen, C.byref(fmax))
+        settings = (noise_scale_w, length_scale, sdp_ratio, item_noise_scale)
+        if all(not isinstance(v, torch.Tensor) for v in settings):
+            self._check(self.lib.bv2_infer_begin(*head, float(noise_scale_w), float(length_scale), float(sdp_ratio), *tail))
+        else:
+            arrays = [self._items(v, B) for v in settings[:3]] + [self._items(1.0 if item_noise_scale is None else item_noise_scale, B)]
+            self._keep += arrays
+            self._check(self.lib.bv2_infer_begin_items(*head, *(_ptr(a) for a in arrays), *tail))
         return np.frombuffer(ylen, dtype=np.int64).copy(), int(fmax.value)
+
+    def _items(self, v, B):
+        """a setting as the fp32 [B] device array bv2_infer_begin_items takes: a float broadcast, or a tensor of B values"""
+        if not isinstance(v, torch.Tensor):
+            return torch.full((B,), float(v), device=self.device, dtype=torch.float32)
+        if v.shape != (B,):
+            raise ValueError(f"a per-utterance setting must have shape [{B}], got {list(v.shape)}")
+        return self._f32(v)
 
     def infer_finish(self, B, T, F, noise_z, noise_scale, max_len=None, want_attn=True, out_ptr: Optional[int] = None, pcm16: bool = False,
                      ragged: bool = False):

@@ -35,23 +35,42 @@ def pad_items(items: Sequence[Tuple[torch.Tensor, ...]], device) -> dict:
     return {k: v.to(device, non_blocking=True) for k, v in out.items()}
 
 
+def _per_item(name, v, n):
+    """v as a list of n per-item values, or None when it is one value for every item"""
+    if np.ndim(v) == 0:
+        return None
+    vals = v.tolist() if hasattr(v, "tolist") else list(v)
+    if len(vals) != n or any(np.ndim(x) != 0 for x in vals):
+        raise ValueError(f"{name}: expected one value or {n} per-item values in item order")
+    return vals
+
+
 @torch.no_grad()
-def infer_batch(net, items: Sequence[Tuple[torch.Tensor, ...]], sid: int, batch_size: int = 32, sdp_ratio=0.2, noise_scale=0.6,
+def infer_batch(net, items: Sequence[Tuple[torch.Tensor, ...]], sid, batch_size: int = 32, sdp_ratio=0.2, noise_scale=0.6,
                 noise_scale_w=0.8, length_scale=1.0, ragged=False) -> List[np.ndarray]:
     """Returns one float32 waveform per item (same order), as infer.infer returns for a single slice (infer.py:315-318).
     `ragged=True` is passed to net.infer: the Generator then runs each utterance at its own length, so no utterance pays for the
-    longest one of its bucket and none sees the padding in its last frames (FP16 Generator only; see SynthesizerTrn.infer)."""
+    longest one of its bucket and none sees the padding in its last frames (FP16 Generator only; see SynthesizerTrn.infer).
+    `sid` and each setting take one value for every item or a sequence of per-item values in item order (a webui dialogue whose
+    sentences have their own speaker and speed).  Buckets depend on the lengths alone, so items with different speakers or settings
+    share a call, each synthesised with its own values (SynthesizerTrn.infer)."""
     dev = next(net.parameters()).device
     lengths = [int(it[3].shape[0]) for it in items]
+    settings = dict(sdp_ratio=sdp_ratio, noise_scale=noise_scale, noise_scale_w=noise_scale_w, length_scale=length_scale)
+    per_item = {k: _per_item(k, v, len(items)) for k, v in settings.items()}
+    sid_items = _per_item("sid", sid, len(items))
     plan = deal_buckets(lengths, world_size=1, batch_size=batch_size)[0]
     hop = net.cfg.hop
     results: List[np.ndarray] = [None] * len(items)
     for bucket in plan:
         d = pad_items([items[i] for i in bucket], dev)
-        sids = torch.full((len(bucket),), int(sid), dtype=torch.int64, device=dev)
+        if sid_items is None:
+            sids = torch.full((len(bucket),), int(sid), dtype=torch.int64, device=dev)
+        else:
+            sids = torch.tensor([int(sid_items[i]) for i in bucket], dtype=torch.int64, device=dev)
+        kw = {k: v if per_item[k] is None else [per_item[k][i] for i in bucket] for k, v in settings.items()}
         o, _, y_mask, _ = net.infer(d["x"], d["x_lengths"], sids, d["tone"], d["language"], d["bert"], d["ja_bert"], d["en_bert"],
-                                    sdp_ratio=sdp_ratio, noise_scale=noise_scale, noise_scale_w=noise_scale_w, length_scale=length_scale,
-                                    ragged=ragged)
+                                    **kw, ragged=ragged)
         n = (y_mask.sum((1, 2)).long() * hop).cpu()
         wav = o[:, 0].float().cpu().numpy()
         for k, i in enumerate(bucket):

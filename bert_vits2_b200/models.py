@@ -19,6 +19,7 @@ import contextlib
 import threading
 from typing import Optional
 
+import numpy as np
 import torch
 from torch import nn
 
@@ -28,6 +29,25 @@ from .pool import EnginePool
 from .spec import ModelConfig, param_specs
 
 _ENGINE_LOCK = threading.Lock()  # builds a module's engine and pool once when several threads make its first call together
+
+
+def item_settings(B: int, **settings):
+    """Each synthesis setting of infer() / infer_stream() as a float, or as an fp32 [B] tensor (on the device it came from) when
+    it is given per utterance as a 1-D sequence or tensor of B values.  A 0-d tensor counts as a float.  Another length or rank
+    raises ValueError."""
+    out = {}
+    for name, v in settings.items():
+        try:
+            if np.ndim(v) == 0:
+                out[name] = float(v)
+                continue
+            t = v.to(torch.float32) if isinstance(v, torch.Tensor) else torch.as_tensor(v, dtype=torch.float32)
+        except (TypeError, ValueError, RuntimeError) as e:
+            raise ValueError(f"{name}: expected a float or {B} per-utterance values") from e
+        if t.dim() != 1 or t.shape[0] != B:
+            raise ValueError(f"{name}: expected a float or {B} per-utterance values, got shape {list(t.shape)}")
+        out[name] = t
+    return out
 
 
 class _Lane:
@@ -210,6 +230,22 @@ class SynthesizerTrn(nn.Module):
             raise Bv2Error(f"SynthesizerTrn.{what}: module is on CPU; bert_vits2_b200 has no CPU path — call .to('cuda')")
         return dev
 
+    def _begin(self, eng, dev, results, args, noise_w, settings, w_ceil_override):
+        """eng.infer_begin with `settings` (item_settings) -> (y_lengths, F, the noise_scale infer_finish* takes).  Per-utterance
+        settings go to the device and to `results`, and a per-utterance noise_scale becomes item_noise_scale (finish then takes 1.0)."""
+        s = dict(settings)
+        if all(not isinstance(v, torch.Tensor) for v in s.values()):  # the scalar call
+            y_lengths, F = eng.infer_begin(*args, noise_w, s["noise_scale_w"], s["length_scale"], s["sdp_ratio"], w_ceil_override)
+            return y_lengths, F, s["noise_scale"]
+        for k, v in s.items():
+            if isinstance(v, torch.Tensor):
+                s[k] = v.to(device=dev, dtype=torch.float32).contiguous()
+                results.append(s[k])
+        ns = s["noise_scale"]
+        y_lengths, F = eng.infer_begin(*args, noise_w, s["noise_scale_w"], s["length_scale"], s["sdp_ratio"], w_ceil_override,
+                                       item_noise_scale=ns if isinstance(ns, torch.Tensor) else None)
+        return y_lengths, F, 1.0 if isinstance(ns, torch.Tensor) else ns
+
     # ----------------------------------------------------------------------------------------------------
     @torch.no_grad()
     def infer(self, x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_scale=0.667, length_scale=1,
@@ -222,9 +258,14 @@ class SynthesizerTrn(nn.Module):
         ValueError otherwise): the Generator runs each utterance at its own length instead of the padded one, so each waveform is
         what the utterance gives alone (its last frames do not see the padding) and 0 past its length; a different result from
         the reference's padded batch, not a faster route to it.  `attn` comes back as a LazyAttn (see above).
+        noise_scale, length_scale, noise_scale_w and sdp_ratio each take a float, as in the reference, which only takes scalars, or a
+        1-D sequence or tensor of B values, one per utterance (ValueError for another length or rank): utterance b then comes out
+        bit-identical to a call of the same batch with its own values as floats, at the launches of one call.
         The call leases one engine of the module's pool from begin to finish (concurrency=N: up to N calls run at once)."""
         if ragged and self.precision not in ("fp16", "fp16g"):
             raise ValueError(f"ragged=True needs the FP16 Generator (precision fp16 or fp16g), not {self.precision}")
+        settings = item_settings(x.shape[0], noise_scale=noise_scale, length_scale=length_scale, noise_scale_w=noise_scale_w,
+                                 sdp_ratio=sdp_ratio)
         dev = self._cuda_device("infer")
         if x.dim() != 2 or bert.dim() != 3 or bert.shape[-1] != x.shape[1]:
             raise ValueError("expected x [B,T] and bert features [B,1024,T]")
@@ -234,8 +275,8 @@ class SynthesizerTrn(nn.Module):
             with _Lane(eng, self.concurrency > 1).step() as results:
                 if noise_w is None:  # same draw order/shape as the reference: SDP first (models.py:249)
                     noise_w = torch.randn(B, 2, T, device=dev, dtype=torch.float32)
-                y_lengths, F = eng.infer_begin(x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_w, noise_scale_w,
-                                               length_scale, sdp_ratio, w_ceil_override)
+                y_lengths, F, noise_scale = self._begin(eng, dev, results, (x, x_lengths, sid, tone, language, bert, ja_bert, en_bert),
+                                                        noise_w, settings, w_ceil_override)
                 if noise_z is None:  # torch.randn_like(m_p), m_p: [B, inter, F] (models.py:1071)
                     noise_z = torch.randn(B, self.inter_channels, F, device=dev, dtype=torch.float32)
                 extra = {"ragged": True} if ragged else {}
@@ -262,9 +303,12 @@ class SynthesizerTrn(nn.Module):
         double without limit and every Generator activation stays resident until the stream ends.
         `ragged=True` (precision fp16 / fp16g only, ValueError otherwise): the Generator runs each utterance at its own length, as
         infer(..., ragged=True) does, with the same chunks.  Utterance b's samples are final and complete once a chunk ends at or past
-        last_y_lengths[b] * hop (max_len applied), and the concatenation is bit-identical to infer(..., ragged=True)[0]: 0 past its end."""
+        last_y_lengths[b] * hop (max_len applied), and the concatenation is bit-identical to infer(..., ragged=True)[0]: 0 past its end.
+        The four synthesis settings take a float (the reference only takes scalars) or B per-utterance values, as in infer()."""
         if ragged and self.precision not in ("fp16", "fp16g"):
             raise ValueError(f"ragged=True needs the FP16 Generator (precision fp16 or fp16g), not {self.precision}")
+        settings = item_settings(x.shape[0], noise_scale=noise_scale, length_scale=length_scale, noise_scale_w=noise_scale_w,
+                                 sdp_ratio=sdp_ratio)
         dev = self._cuda_device("infer_stream")
         if x.dim() != 2 or bert.dim() != 3 or bert.shape[-1] != x.shape[1]:
             raise ValueError("expected x [B,T] and bert features [B,1024,T]")
@@ -280,8 +324,8 @@ class SynthesizerTrn(nn.Module):
             with lane.step() as results:
                 if noise_w is None:
                     noise_w = torch.randn(B, 2, T, device=dev, dtype=torch.float32)
-                y_lengths, F = eng.infer_begin(x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_w, noise_scale_w,
-                                               length_scale, sdp_ratio, w_ceil_override)
+                y_lengths, F, noise_scale = self._begin(eng, dev, results, (x, x_lengths, sid, tone, language, bert, ja_bert, en_bert),
+                                                        noise_w, settings, w_ceil_override)
                 if noise_z is None:
                     noise_z = torch.randn(B, self.inter_channels, F, device=dev, dtype=torch.float32)
                 extra = {} if max_chunk_frames is None else {"max_chunk_frames": max_chunk_frames}

@@ -99,6 +99,20 @@ int bv2_infer_begin(bv2_engine* e, int B, int T, const int64_t* x, const int64_t
                     const float* en_bert, const float* noise_w, float noise_scale_w, float length_scale,
                     float sdp_ratio, const float* w_ceil_override, void* stream, int64_t* y_lengths_host,
                     int32_t* f_max);
+/* Per-utterance settings: bv2_infer_begin, except that noise_scale_w, length_scale and sdp_ratio are DEVICE fp32 arrays [B] and
+ * utterance b is synthesised with its own entries, and that noise_scale [B] (DEVICE fp32) gives each utterance its own prior-noise
+ * scale.  Every bv2_infer_finish* that follows samples utterance b with noise_scale_arg * noise_scale[b] rounded once to fp32, where
+ * noise_scale_arg is the finish call's own noise_scale: pass 1.0 there to get exactly noise_scale[b].  bv2_infer_begin clears the
+ * per-utterance scale, so after it finish uses noise_scale_arg alone.  Each setting only scales per-utterance elementwise arithmetic,
+ * so utterance b's outputs (durations, y_lengths and, for the same F, everything finish writes) are bit-identical to those of the
+ * same batch begun by bv2_infer_begin with b's settings as scalars.  Same launches, host read-back and workspace as bv2_infer_begin;
+ * the engine copies noise_scale before returning, so the caller may free the four arrays after the call.  A NULL array returns
+ * BV2_ERR_ARG. */
+int bv2_infer_begin_items(bv2_engine* e, int B, int T, const int64_t* x, const int64_t* x_lengths, const int64_t* sid,
+                          const int64_t* tone, const int64_t* language, const float* bert, const float* ja_bert,
+                          const float* en_bert, const float* noise_w, const float* noise_scale_w, const float* length_scale,
+                          const float* sdp_ratio, const float* noise_scale, const float* w_ceil_override, void* stream,
+                          int64_t* y_lengths_host, int32_t* f_max);
 
 /* finish: length regulation -> prior sample -> flow reverse -> Generator.  noise_z [B,inter,>=F] with row stride
  * noise_ld replaces torch.randn_like at models.py:1071.  Outputs (caller-allocated, any may be NULL except o):
