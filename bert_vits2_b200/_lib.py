@@ -60,6 +60,8 @@ SYMBOLS = {
                                   C.c_float, C.c_float, F32P, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
     "bv2_infer_begin_items": (C.c_int, [P, C.c_int, C.c_int, I64P, I64P, I64P, I64P, I64P, F32P, F32P, F32P, F32P, F32P, F32P, F32P,
                                         F32P, F32P, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
+    "bv2_infer_begin_mix": (C.c_int, [P, C.c_int, C.c_int, I64P, I64P, C.c_int, I64P, F32P, I64P, I64P, F32P, F32P, F32P, F32P, F32P, F32P,
+                                      F32P, F32P, F32P, C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
     "bv2_infer_finish": (C.c_int, [P, F32P, C.c_int64, C.c_float, C.c_int32, F32P, F32P, F32P, F32P, F32P, F32P, F32P, C.c_void_p]),
     "bv2_infer_finish_pcm16": (C.c_int, [P, F32P, C.c_int64, C.c_float, C.c_int32, C.c_void_p, F32P, F32P, F32P, F32P, F32P, F32P, C.c_void_p]),
     "bv2_infer_finish_ragged": (C.c_int, [P, F32P, C.c_int64, C.c_float, C.c_int32, F32P, C.c_void_p, F32P, F32P, F32P, F32P, F32P, F32P,

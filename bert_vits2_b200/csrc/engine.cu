@@ -427,12 +427,15 @@ struct bv2_engine : DeviceWeights {
     }
     static void throw_if_bad_inputs(int mask) {
         if (!mask) return;
+        const char* weight = "non-finite speaker-mix weight";
+        if (!(mask & 31)) throw Error(BV2_ERR_ARG, weight);  // no "index out of range": a ValueError in Python, not an IndexError
         std::string m = "index out of range:";
         if (mask & 1) m += " phoneme id (n_vocab)";
         if (mask & 2) m += " tone id";
         if (mask & 4) m += " language id";
         if (mask & 8) m += " speaker id (n_speakers)";
         if (mask & 16) m += " x_lengths (need 1 <= len <= T)";
+        if (mask & 32) m += std::string("; ") + weight;
         throw Error(BV2_ERR_ARG, m);
     }
     // stage entry points (not on the hot path): validate, read the verdict back synchronously
@@ -1468,18 +1471,22 @@ int bv2_load_packed(bv2_engine* e, const char* path) {
 
 // items: the settings are per-item device arrays [B] (bv2_infer_begin_items) instead of the scalars, which are then ignored
 struct ItemSettings { const float *noise_scale_w, *length_scale, *sdp_ratio, *noise_scale; };
+// mix: g is each item's weighted sum of K emb_g rows (bv2_infer_begin_mix) instead of the row of sid, which is then ignored
+struct SpeakerMix { int K; const int64_t* sid; const float* weight; };
 
 static int infer_begin_impl(bv2_engine* e, int B, int T, const int64_t* x, const int64_t* x_lengths, const int64_t* sid,
                             const int64_t* tone, const int64_t* language, const float* bert, const float* ja_bert,
                             const float* en_bert, const float* noise_w, float noise_scale_w, float length_scale, float sdp_ratio,
                             const ItemSettings* items, const float* w_ceil_override, void* stream, int64_t* y_lengths_host,
-                            int32_t* f_max) {
+                            int32_t* f_max, const SpeakerMix* mix = nullptr) {
     BV2_API_BEGIN(e)
     BV2_CHECK(e->finalized, "not finalized");
-    BV2_CHECK(B >= 1 && B <= 4096 && T >= 1 && x && x_lengths && sid && tone && language && bert && ja_bert && en_bert && noise_w &&
-                  y_lengths_host && f_max, "infer_begin args");
+    BV2_CHECK(B >= 1 && B <= 4096 && T >= 1 && x && x_lengths && (sid || mix) && tone && language && bert && ja_bert && en_bert &&
+                  noise_w && y_lengths_host && f_max, "infer_begin args");
     if (items && !(items->noise_scale_w && items->length_scale && items->sdp_ratio && items->noise_scale))
         throw Error(BV2_ERR_ARG, "infer_begin_items: every setting array must be given");
+    if (mix && !(mix->K >= 1 && (int64_t)B * mix->K <= INT32_MAX && mix->sid && mix->weight))
+        throw Error(BV2_ERR_ARG, "infer_begin_mix: need K >= 1, B*K <= INT32_MAX and both mix arrays");
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const bv2_config& c = e->cfg;
     const int H = c.hidden_channels, I = c.inter_channels;
@@ -1498,12 +1505,17 @@ static int infer_begin_impl(bv2_engine* e, int B, int T, const int64_t* x, const
         st.noise_scale = e->persist.alloc(B);
         BV2_CUDA(cudaMemcpyAsync(st.noise_scale, items->noise_scale, (size_t)B * sizeof(float), cudaMemcpyDeviceToDevice, s));
     }
-    e->launch_validate(B, T, x, tone, language, sid, x_lengths, err_dev, s);
+    e->launch_validate(B, T, x, tone, language, mix ? nullptr : sid, x_lengths, err_dev, s);  // k_speaker_mix checks a mix's ids
     st.lens = e->lens_to_device(x_lengths, B, e->persist, s);
     float* g = e->persist.alloc((size_t)B * c.gin_channels);
     st.gproj = e->persist.alloc((size_t)B * e->gproj_n);
-    k_gather_rows<<<B, 128, 0, s>>>(e->emb_g, reinterpret_cast<const long long*>(sid), g, c.gin_channels, c.n_speakers);
+    if (mix)
+        k_speaker_mix<<<B, 128, 0, s>>>(e->emb_g, reinterpret_cast<const long long*>(mix->sid), mix->weight, mix->K, g, c.gin_channels,
+                                        c.n_speakers, err_dev);
+    else
+        k_gather_rows<<<B, 128, 0, s>>>(e->emb_g, reinterpret_cast<const long long*>(sid), g, c.gin_channels, c.n_speakers);
     BV2_CUDA(cudaGetLastError()); e->launches++;
+    e->debug_plain("g", g, B, c.gin_channels, 1);
     e->run_gproj(g, B, st.gproj, s);
     Act h = e->ws.act(B, H, T);
     Act stats; stats.B = B; stats.C = 2 * I; stats.T = T; stats.p = e->persist.alloc(stats.elems());
@@ -1550,6 +1562,17 @@ int bv2_infer_begin_items(bv2_engine* e, int B, int T, const int64_t* x, const i
     const ItemSettings items{noise_scale_w, length_scale, sdp_ratio, noise_scale};
     return infer_begin_impl(e, B, T, x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_w, 1.f, 1.f, 0.f, &items,
                             w_ceil_override, stream, y_lengths_host, f_max);
+}
+
+int bv2_infer_begin_mix(bv2_engine* e, int B, int T, const int64_t* x, const int64_t* x_lengths, int K, const int64_t* mix_sid,
+                        const float* mix_weight, const int64_t* tone, const int64_t* language, const float* bert, const float* ja_bert,
+                        const float* en_bert, const float* noise_w, const float* noise_scale_w, const float* length_scale,
+                        const float* sdp_ratio, const float* noise_scale, const float* w_ceil_override, void* stream,
+                        int64_t* y_lengths_host, int32_t* f_max) {
+    const ItemSettings items{noise_scale_w, length_scale, sdp_ratio, noise_scale};
+    const SpeakerMix mix{K, mix_sid, mix_weight};
+    return infer_begin_impl(e, B, T, x, x_lengths, nullptr, tone, language, bert, ja_bert, en_bert, noise_w, 1.f, 1.f, 0.f, &items,
+                            w_ceil_override, stream, y_lengths_host, f_max, &mix);
 }
 
 // open_stream: stop after the flow and open a Generator stream over o instead of running the Generator (bv2_infer_finish_stream)

@@ -417,10 +417,36 @@ __global__ void k_gather_rows(const float* __restrict__ table, const long long* 
     for (int i = threadIdx.x; i < C; i += blockDim.x) out[(size_t)b * C + i] = table[(size_t)r * C + i];
 }
 
+// Speaker mix (bv2_infer_begin_mix): out[b][c] = sum_k w[b][k] * table[id[b][k]][c], summed in k order with one fp32 rounding per
+// product and per sum (__fmul_rn / __fadd_rn: no FMA contraction, so np.float32 in the same order gives the same bits).  One block
+// per b.  Validates the mix like k_validate_inputs: ORs 8 into *err for an id outside [0, nrows) (the read is clamped) and 32 for
+// a non-finite weight.
+__global__ void k_speaker_mix(const float* __restrict__ table, const long long* __restrict__ ids, const float* __restrict__ w, int K,
+                              float* __restrict__ out, int C, int nrows, int* __restrict__ err) {
+    const int b = blockIdx.x;
+    const long long* id = ids + (size_t)b * K;
+    const float* wb = w + (size_t)b * K;
+    int bad = 0;
+    for (int i = threadIdx.x; i < C; i += blockDim.x) {
+        float acc = 0.f;
+        for (int k = 0; k < K; k++) {
+            const long long r = id[k];
+            const float wk = wb[k];
+            if (r < 0 || r >= nrows) bad |= 8;
+            if (!isfinite(wk)) bad |= 32;
+            const float p = __fmul_rn(wk, table[(size_t)min(max(r, 0ll), (long long)nrows - 1) * C + i]);
+            acc = k ? __fadd_rn(acc, p) : p;
+        }
+        out[(size_t)b * C + i] = acc;
+    }
+    if (bad && threadIdx.x == 0) atomicOr(err, bad);  // thread 0 walks every k for channel 0
+}
+
 // Input validation (the reference raises IndexError from nn.Embedding / a shape error for bad lengths; reference
 // models.py:378-384, 1046): ids must lie inside their tables and 1 <= x_lengths[b] <= T.  Writes a bit mask into *err
 // (read back together with y_lengths: no extra synchronisation): 1 = phoneme id, 2 = tone, 4 = language, 8 = speaker id,
-// 16 = x_lengths.  Gather kernels clamp, so a bad id can never become an out-of-bounds access.
+// 16 = x_lengths (32 = a non-finite speaker-mix weight, from k_speaker_mix).  Gather kernels clamp, so a bad id can never become
+// an out-of-bounds access.
 __global__ void k_validate_inputs(const long long* __restrict__ x, const long long* __restrict__ tone, const long long* __restrict__ lang,
                                   const long long* __restrict__ sid, const long long* __restrict__ lens, int B, int T, int n_vocab,
                                   int n_tones, int n_langs, int n_spk, int* __restrict__ err) {

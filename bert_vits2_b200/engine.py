@@ -169,13 +169,18 @@ class Engine:
 
     # ---- whole path ---------------------------------------------------------------------------------
     def infer_begin(self, x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_w, noise_scale_w, length_scale,
-                    sdp_ratio, w_ceil_override=None, *, item_noise_scale=None):
+                    sdp_ratio, w_ceil_override=None, *, item_noise_scale=None, speaker_mix=None):
         """noise_scale_w, length_scale and sdp_ratio: a float, or a [B] tensor of per-utterance values.  `item_noise_scale` [B]: each
         utterance's prior-noise scale, multiplied (rounded once) into the noise_scale every infer_finish* takes, so pass 1.0 there.
         With any tensor this is bv2_infer_begin_items (floats broadcast to [B], item_noise_scale 1.0 when None), and utterance b comes
-        out bit-identical to a call with its own values as floats; with floats alone it is bv2_infer_begin."""
+        out bit-identical to a call with its own values as floats; with floats alone it is bv2_infer_begin.
+        `speaker_mix` (ids [B,K] int64, weights [B,K] fp32), with sid None: utterance b is conditioned on sum_k weights[b,k] *
+        emb_g[ids[b,k]] in k order instead of one speaker's row (bv2_infer_begin_mix, the settings broadcast as for
+        bv2_infer_begin_items)."""
         B, T = x.shape
-        self._keep = [self._i64(x), self._i64(x_lengths), self._i64(sid), self._i64(tone), self._i64(language),
+        if (sid is None) == (speaker_mix is None):
+            raise ValueError("infer_begin takes either sid or speaker_mix")
+        self._keep = [self._i64(x), self._i64(x_lengths), None if sid is None else self._i64(sid), self._i64(tone), self._i64(language),
                       self._f32(bert), self._f32(ja_bert), self._f32(en_bert), self._f32(noise_w),
                       None if w_ceil_override is None else self._f32(w_ceil_override)]
         k = self._keep
@@ -184,12 +189,20 @@ class Engine:
         head = (self._h, B, T, *(_ptr(t) for t in k[:9]))
         tail = (_ptr(k[9]), self._stream(), ylen, C.byref(fmax))
         settings = (noise_scale_w, length_scale, sdp_ratio, item_noise_scale)
-        if all(not isinstance(v, torch.Tensor) for v in settings):
+        if speaker_mix is None and all(not isinstance(v, torch.Tensor) for v in settings):
             self._check(self.lib.bv2_infer_begin(*head, float(noise_scale_w), float(length_scale), float(sdp_ratio), *tail))
-        else:
-            arrays = [self._items(v, B) for v in settings[:3]] + [self._items(1.0 if item_noise_scale is None else item_noise_scale, B)]
-            self._keep += arrays
+            return np.frombuffer(ylen, dtype=np.int64).copy(), int(fmax.value)
+        arrays = [self._items(v, B) for v in settings[:3]] + [self._items(1.0 if item_noise_scale is None else item_noise_scale, B)]
+        self._keep += arrays
+        if speaker_mix is None:
             self._check(self.lib.bv2_infer_begin_items(*head, *(_ptr(a) for a in arrays), *tail))
+        else:
+            ids, w = self._i64(speaker_mix[0]), self._f32(speaker_mix[1])
+            if ids.dim() != 2 or ids.shape[0] != B or ids.shape != w.shape:
+                raise ValueError(f"speaker_mix: expected ids and weights of one shape [{B}, K], got {list(ids.shape)} and {list(w.shape)}")
+            self._keep += [ids, w]
+            self._check(self.lib.bv2_infer_begin_mix(self._h, B, T, _ptr(k[0]), _ptr(k[1]), ids.shape[1], _ptr(ids), _ptr(w),
+                                                     *(_ptr(t) for t in k[3:9]), *(_ptr(a) for a in arrays), *tail))
         return np.frombuffer(ylen, dtype=np.int64).copy(), int(fmax.value)
 
     def _items(self, v, B):

@@ -14,6 +14,7 @@ from typing import List, Sequence, Tuple
 import numpy as np
 import torch
 
+from .models import speaker_mixes
 from .sharding import deal_buckets
 
 
@@ -46,29 +47,40 @@ def _per_item(name, v, n):
 
 
 @torch.no_grad()
-def infer_batch(net, items: Sequence[Tuple[torch.Tensor, ...]], sid, batch_size: int = 32, sdp_ratio=0.2, noise_scale=0.6,
-                noise_scale_w=0.8, length_scale=1.0, ragged=False) -> List[np.ndarray]:
+def infer_batch(net, items: Sequence[Tuple[torch.Tensor, ...]], sid=None, batch_size: int = 32, sdp_ratio=0.2, noise_scale=0.6,
+                noise_scale_w=0.8, length_scale=1.0, ragged=False, speaker_mix=None) -> List[np.ndarray]:
     """Returns one float32 waveform per item (same order), as infer.infer returns for a single slice (infer.py:315-318).
     `ragged=True` is passed to net.infer: the Generator then runs each utterance at its own length, so no utterance pays for the
     longest one of its bucket and none sees the padding in its last frames (FP16 Generator only; see SynthesizerTrn.infer).
     `sid` and each setting take one value for every item or a sequence of per-item values in item order (a webui dialogue whose
     sentences have their own speaker and speed).  Buckets depend on the lengths alone, so items with different speakers or settings
-    share a call, each synthesised with its own values (SynthesizerTrn.infer)."""
+    share a call, each synthesised with its own values (SynthesizerTrn.infer).
+    `speaker_mix` replaces `sid` (ValueError with both, or with neither): one dict {speaker_id: weight} for every item or one dict
+    per item in item order, each item conditioned on its own weighted mix of speakers (models.speaker_mixes)."""
     dev = next(net.parameters()).device
     lengths = [int(it[3].shape[0]) for it in items]
     settings = dict(sdp_ratio=sdp_ratio, noise_scale=noise_scale, noise_scale_w=noise_scale_w, length_scale=length_scale)
     per_item = {k: _per_item(k, v, len(items)) for k, v in settings.items()}
-    sid_items = _per_item("sid", sid, len(items))
+    if (sid is None) == (speaker_mix is None):
+        raise ValueError("infer_batch takes either sid or speaker_mix")
+    if speaker_mix is None:
+        sid_items = _per_item("sid", sid, len(items))
+    else:
+        speaker_mixes(len(items), speaker_mix)  # validates every mix before the first call
+        mixes = [speaker_mix] * len(items) if isinstance(speaker_mix, dict) else list(speaker_mix)
     plan = deal_buckets(lengths, world_size=1, batch_size=batch_size)[0]
     hop = net.cfg.hop
     results: List[np.ndarray] = [None] * len(items)
     for bucket in plan:
         d = pad_items([items[i] for i in bucket], dev)
-        if sid_items is None:
+        kw = {k: v if per_item[k] is None else [per_item[k][i] for i in bucket] for k, v in settings.items()}
+        if speaker_mix is not None:
+            sids = None
+            kw["speaker_mix"] = [mixes[i] for i in bucket]
+        elif sid_items is None:
             sids = torch.full((len(bucket),), int(sid), dtype=torch.int64, device=dev)
         else:
             sids = torch.tensor([int(sid_items[i]) for i in bucket], dtype=torch.int64, device=dev)
-        kw = {k: v if per_item[k] is None else [per_item[k][i] for i in bucket] for k, v in settings.items()}
         o, _, y_mask, _ = net.infer(d["x"], d["x_lengths"], sids, d["tone"], d["language"], d["bert"], d["ja_bert"], d["en_bert"],
                                     **kw, ragged=ragged)
         n = (y_mask.sum((1, 2)).long() * hop).cpu()

@@ -50,6 +50,43 @@ def item_settings(B: int, **settings):
     return out
 
 
+def speaker_mixes(B: int, mix):
+    """A speaker mix of infer() / infer_stream() as the (ids [B,K] int64, weights [B,K] fp32) CPU tensors Engine.infer_begin takes.
+    `mix`: one dict {speaker_id: weight} for every utterance, or a sequence of B such dicts.  Dict order is summation order; a
+    shorter mix is padded at the end to the batch's K with (its first id, 0.0).  Weights are used as given.  An empty dict, a
+    non-integer or bool key, a non-finite weight or a sequence whose length is not B raises ValueError."""
+    if isinstance(mix, dict):
+        mixes = [mix] * B
+    else:
+        try:
+            mixes = list(mix)
+        except TypeError as e:
+            raise ValueError("speaker_mix: expected a dict {speaker_id: weight} or a sequence of one per utterance") from e
+        if len(mixes) != B:
+            raise ValueError(f"speaker_mix: expected one dict or {B} dicts, got {len(mixes)}")
+    rows = []
+    for m in mixes:
+        if not isinstance(m, dict) or not m:
+            raise ValueError("speaker_mix: each mix must be a non-empty dict {speaker_id: weight}")
+        ids = list(m.keys())
+        if any(isinstance(i, (bool, np.bool_)) or not isinstance(i, (int, np.integer)) for i in ids):
+            raise ValueError(f"speaker_mix: speaker ids must be integers, got {ids}")
+        try:
+            w = torch.tensor([float(v) for v in m.values()], dtype=torch.float32)
+        except (TypeError, ValueError) as e:
+            raise ValueError("speaker_mix: weights must be numbers") from e
+        if not torch.isfinite(w).all():
+            raise ValueError(f"speaker_mix: weights must be finite in fp32, got {list(m.values())}")
+        rows.append(([int(i) for i in ids], w))
+    K = max(len(ids) for ids, _ in rows)
+    out_ids = torch.empty(B, K, dtype=torch.int64)
+    out_w = torch.zeros(B, K, dtype=torch.float32)
+    for b, (ids, w) in enumerate(rows):
+        out_ids[b] = torch.tensor(ids + [ids[0]] * (K - len(ids)))
+        out_w[b, :len(ids)] = w
+    return out_ids, out_w
+
+
 class _Lane:
     """Where a leased engine's work runs.  Without an own stream (concurrency=1): on the caller's current stream, as a single engine
     always ran.  With one: on the engine's own stream, which waits for the caller's work before each step; after the step the caller's
@@ -230,27 +267,40 @@ class SynthesizerTrn(nn.Module):
             raise Bv2Error(f"SynthesizerTrn.{what}: module is on CPU; bert_vits2_b200 has no CPU path — call .to('cuda')")
         return dev
 
-    def _begin(self, eng, dev, results, args, noise_w, settings, w_ceil_override):
-        """eng.infer_begin with `settings` (item_settings) -> (y_lengths, F, the noise_scale infer_finish* takes).  Per-utterance
-        settings go to the device and to `results`, and a per-utterance noise_scale becomes item_noise_scale (finish then takes 1.0)."""
+    def _begin(self, eng, dev, results, args, noise_w, settings, w_ceil_override, mix=None):
+        """eng.infer_begin with `settings` (item_settings) and `mix` (speaker_mixes, or None) -> (y_lengths, F, the noise_scale
+        infer_finish* takes).  Per-utterance settings and the mix go to the device and to `results`, and a per-utterance noise_scale
+        becomes item_noise_scale (finish then takes 1.0)."""
         s = dict(settings)
-        if all(not isinstance(v, torch.Tensor) for v in s.values()):  # the scalar call
+        if mix is None and all(not isinstance(v, torch.Tensor) for v in s.values()):  # the scalar call
             y_lengths, F = eng.infer_begin(*args, noise_w, s["noise_scale_w"], s["length_scale"], s["sdp_ratio"], w_ceil_override)
             return y_lengths, F, s["noise_scale"]
         for k, v in s.items():
             if isinstance(v, torch.Tensor):
                 s[k] = v.to(device=dev, dtype=torch.float32).contiguous()
                 results.append(s[k])
+        if mix is not None:
+            mix = tuple(t.to(device=dev).contiguous() for t in mix)
+            results += mix
         ns = s["noise_scale"]
         y_lengths, F = eng.infer_begin(*args, noise_w, s["noise_scale_w"], s["length_scale"], s["sdp_ratio"], w_ceil_override,
-                                       item_noise_scale=ns if isinstance(ns, torch.Tensor) else None)
+                                       item_noise_scale=ns if isinstance(ns, torch.Tensor) else None, speaker_mix=mix)
         return y_lengths, F, 1.0 if isinstance(ns, torch.Tensor) else ns
+
+    @staticmethod
+    def _mix(B, sid, speaker_mix):
+        """speaker_mix as speaker_mixes gives it, or None; ValueError when it comes with a sid"""
+        if speaker_mix is None:
+            return None
+        if sid is not None:
+            raise ValueError("give either sid or speaker_mix, not both (pass sid=None with a speaker mix)")
+        return speaker_mixes(B, speaker_mix)
 
     # ----------------------------------------------------------------------------------------------------
     @torch.no_grad()
     def infer(self, x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_scale=0.667, length_scale=1,
               noise_scale_w=0.8, max_len=None, sdp_ratio=0, y=None, *, noise_w=None, noise_z=None, w_ceil_override=None, pcm16=False,
-              ragged=False):
+              ragged=False, speaker_mix=None):
         """reference models.py:1026-1074.  Keyword-only extras (not in the reference): explicit noise tensors
         `noise_w` [B,2,T] / `noise_z` [B,inter,>=F] replacing the two in-model RNG draws (models.py:249, 1071), and
         `w_ceil_override` [B,T] to teacher-force durations in parity harnesses, `pcm16=True` to get `o` as int16 converted like
@@ -261,11 +311,15 @@ class SynthesizerTrn(nn.Module):
         noise_scale, length_scale, noise_scale_w and sdp_ratio each take a float, as in the reference, which only takes scalars, or a
         1-D sequence or tensor of B values, one per utterance (ValueError for another length or rank): utterance b then comes out
         bit-identical to a call of the same batch with its own values as floats, at the launches of one call.
+        `speaker_mix` (with sid=None; ValueError with both): each utterance is conditioned on a weighted sum of speaker embeddings
+        instead of one speaker, given as one dict {speaker_id: weight} for every utterance or a sequence of B dicts (speaker_mixes);
+        utterance b is bit-identical to a plain call on a module whose emb_g holds b's mix as an extra row (bv2_infer_begin_mix).
         The call leases one engine of the module's pool from begin to finish (concurrency=N: up to N calls run at once)."""
         if ragged and self.precision not in ("fp16", "fp16g"):
             raise ValueError(f"ragged=True needs the FP16 Generator (precision fp16 or fp16g), not {self.precision}")
         settings = item_settings(x.shape[0], noise_scale=noise_scale, length_scale=length_scale, noise_scale_w=noise_scale_w,
                                  sdp_ratio=sdp_ratio)
+        mix = self._mix(x.shape[0], sid, speaker_mix)
         dev = self._cuda_device("infer")
         if x.dim() != 2 or bert.dim() != 3 or bert.shape[-1] != x.shape[1]:
             raise ValueError("expected x [B,T] and bert features [B,1024,T]")
@@ -276,7 +330,7 @@ class SynthesizerTrn(nn.Module):
                 if noise_w is None:  # same draw order/shape as the reference: SDP first (models.py:249)
                     noise_w = torch.randn(B, 2, T, device=dev, dtype=torch.float32)
                 y_lengths, F, noise_scale = self._begin(eng, dev, results, (x, x_lengths, sid, tone, language, bert, ja_bert, en_bert),
-                                                        noise_w, settings, w_ceil_override)
+                                                        noise_w, settings, w_ceil_override, mix)
                 if noise_z is None:  # torch.randn_like(m_p), m_p: [B, inter, F] (models.py:1071)
                     noise_z = torch.randn(B, self.inter_channels, F, device=dev, dtype=torch.float32)
                 extra = {"ragged": True} if ragged else {}
@@ -289,7 +343,7 @@ class SynthesizerTrn(nn.Module):
     @torch.no_grad()
     def infer_stream(self, x, x_lengths, sid, tone, language, bert, ja_bert, en_bert, noise_scale=0.667, length_scale=1,
                      noise_scale_w=0.8, max_len=None, sdp_ratio=0, y=None, *, noise_w=None, noise_z=None, w_ceil_override=None,
-                     first_chunk_frames=32, max_chunk_frames=None, ragged=False):
+                     first_chunk_frames=32, max_chunk_frames=None, ragged=False, speaker_mix=None):
         """Streaming infer(): a generator of waveform chunks o[:, :, a:b] (device tensors, views of one [B,1,Fg*hop] buffer) whose
         concatenation is bit-identical to infer(...)[0] with the same noise.  Encoder, durations and flow run whole first (the flow's
         attention spans the utterance); the Generator then runs as a wavefront, so the first chunk costs about first_chunk_frames
@@ -304,11 +358,13 @@ class SynthesizerTrn(nn.Module):
         `ragged=True` (precision fp16 / fp16g only, ValueError otherwise): the Generator runs each utterance at its own length, as
         infer(..., ragged=True) does, with the same chunks.  Utterance b's samples are final and complete once a chunk ends at or past
         last_y_lengths[b] * hop (max_len applied), and the concatenation is bit-identical to infer(..., ragged=True)[0]: 0 past its end.
-        The four synthesis settings take a float (the reference only takes scalars) or B per-utterance values, as in infer()."""
+        The four synthesis settings take a float (the reference only takes scalars) or B per-utterance values, and `speaker_mix` a
+        speaker mix instead of sid, as in infer()."""
         if ragged and self.precision not in ("fp16", "fp16g"):
             raise ValueError(f"ragged=True needs the FP16 Generator (precision fp16 or fp16g), not {self.precision}")
         settings = item_settings(x.shape[0], noise_scale=noise_scale, length_scale=length_scale, noise_scale_w=noise_scale_w,
                                  sdp_ratio=sdp_ratio)
+        mix = self._mix(x.shape[0], sid, speaker_mix)
         dev = self._cuda_device("infer_stream")
         if x.dim() != 2 or bert.dim() != 3 or bert.shape[-1] != x.shape[1]:
             raise ValueError("expected x [B,T] and bert features [B,1024,T]")
@@ -325,7 +381,7 @@ class SynthesizerTrn(nn.Module):
                 if noise_w is None:
                     noise_w = torch.randn(B, 2, T, device=dev, dtype=torch.float32)
                 y_lengths, F, noise_scale = self._begin(eng, dev, results, (x, x_lengths, sid, tone, language, bert, ja_bert, en_bert),
-                                                        noise_w, settings, w_ceil_override)
+                                                        noise_w, settings, w_ceil_override, mix)
                 if noise_z is None:
                     noise_z = torch.randn(B, self.inter_channels, F, device=dev, dtype=torch.float32)
                 extra = {} if max_chunk_frames is None else {"max_chunk_frames": max_chunk_frames}

@@ -113,6 +113,23 @@ int bv2_infer_begin_items(bv2_engine* e, int B, int T, const int64_t* x, const i
                           const float* en_bert, const float* noise_w, const float* noise_scale_w, const float* length_scale,
                           const float* sdp_ratio, const float* noise_scale, const float* w_ceil_override, void* stream,
                           int64_t* y_lengths_host, int32_t* f_max);
+/* Speaker mixes: bv2_infer_begin_items, except that utterance b is conditioned on a weighted mix of K speaker embeddings instead of
+ * the row of one sid.  mix_sid [B,K] (DEVICE int64) and mix_weight [B,K] (DEVICE fp32) give the mix, and
+ *     g[b][c] = fl(w[b][0] * E[id[b][0]][c]),  then for k = 1..K-1:  g[b][c] = fl(g[b][c] + fl(w[b][k] * E[id[b][k]][c]))
+ * with E = emb_g.weight, every operation one fp32 round-to-nearest (no FMA), in k order, so the same loop in IEEE fp32 on the host
+ * gives the same bits.  Weights are used as given (no normalisation; negative weights and any sum allowed); ids may repeat; K is
+ * not bounded by n_speakers.  Everything after g is bv2_infer_begin_items, so utterance b's outputs are bit-identical to those of
+ * the same batch on an engine whose emb_g holds g[b] as an extra row and a plain call with sid = that row; K = 1 with weight 1.0
+ * is bit-identical to bv2_infer_begin_items with sid = id.  Every bv2_infer_finish* that follows inherits the mix.  Same launches,
+ * host read-back and workspace as bv2_infer_begin_items; the mix arrays are only read during the call.  Errors: K < 1,
+ * B*K > INT32_MAX or a NULL array: BV2_ERR_ARG before any work; an id outside [0, n_speakers): BV2_ERR_ARG with "index out of
+ * range: speaker id" in bv2_last_error; a non-finite weight: BV2_ERR_ARG with "non-finite speaker-mix weight" (and the id message
+ * when both occur).  The engine serves the next call normally after any of them. */
+int bv2_infer_begin_mix(bv2_engine* e, int B, int T, const int64_t* x, const int64_t* x_lengths, int K, const int64_t* mix_sid,
+                        const float* mix_weight, const int64_t* tone, const int64_t* language, const float* bert, const float* ja_bert,
+                        const float* en_bert, const float* noise_w, const float* noise_scale_w, const float* length_scale,
+                        const float* sdp_ratio, const float* noise_scale, const float* w_ceil_override, void* stream,
+                        int64_t* y_lengths_host, int32_t* f_max);
 
 /* finish: length regulation -> prior sample -> flow reverse -> Generator.  noise_z [B,inter,>=F] with row stride
  * noise_ld replaces torch.randn_like at models.py:1071.  Outputs (caller-allocated, any may be NULL except o):
